@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — frames/sec of the MIMO denoising path on B200 (BASELINE.json metric).
+"""bench.py — frames/sec of the MIMO denoising path on one H100 (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W]            our engine (one JSON line on rank 0)
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]   our engine (one JSON line on rank 0)
   python bench.py --impl reference [--gpus N] --steps K --warmup W   the oracle port on the host cores
 
 Workload (BASELINE.json configs[1]): 512x512, 24 frames, 20 DDIM steps, CFG 3.5, fp16, synthetic PIL inputs,
@@ -12,8 +12,9 @@ A "step" is one whole clip: Pose2VideoPipeline's work from CLIP/VAE-encode/pose/
 steps to the batched VAE decode. `value` times sample_tensors() with every input already in HBM; `e2e` times the
 public __call__ (PIL in -> CPU video tensor out: PIL pre-processing, pinned H2D, D2H of the clip inside the timed
 region). Inputs differ per step by the noise seed (pre-generated, resident in HBM); the UNet touches > 2.6 GB of
-weights + multi-hundred-MB activations per forward, far beyond the 126 MB L2, so no explicit L2 flush is needed
-between steps.
+weights + multi-hundred-MB activations per forward, far beyond the 50 MB L2, so no explicit L2 flush is needed
+between steps. --dump-outputs DIR writes what the last timed step returned (see dump_outputs) so that two builds can be
+compared output for output: weights, inputs and noise are seeded, so the same arguments give the same inputs.
 
 Both arms print the same `config`. The reference arm times the oracle port (the reference's PyTorch graph, fp32) on the
 host cores: every step is a BOUNDED sample of the workload — one CFG UNet3D forward on f_s of the 24 frames at the full
@@ -48,7 +49,7 @@ TFLOP_PER_FRAME = 49.3
 
 CONFIG = {"workload": "512x512 x 24-frame animate, 20 DDIM steps, CFG 3.5, fp16 (BASELINE.json configs[1])",
           "frames": FRAMES, "ddim_steps": DDIM_STEPS, "guidance_scale": GUIDANCE,
-          "l2": "inputs/weights per forward >> 126 MB L2; no explicit flush"}
+          "l2": "inputs/weights per forward >> 50 MB L2; no explicit flush"}
 DTYPE, DTYPE_NAME, NOISE_BK = torch.float16, "fp16", False
 
 
@@ -71,7 +72,7 @@ def select_config(k: int) -> None:
         raise SystemExit(f"--config {k}: BASELINE.json has configs 1..5 (1 is the CPU plumbing case: tests/)")
     METRIC = f"frames/sec @ {WIDTH}x{HEIGHT}x{FRAMES}f, {DDIM_STEPS} DDIM steps"
     CONFIG = {"workload": name, "frames": FRAMES, "ddim_steps": DDIM_STEPS, "guidance_scale": GUIDANCE,
-              "l2": "inputs/weights per forward >> 126 MB L2; no explicit flush"}
+              "l2": "inputs/weights per forward >> 50 MB L2; no explicit flush"}
 
 SCHED_KW = dict(beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear", clip_sample=False, steps_offset=1,
                 prediction_type="v_prediction", rescale_betas_zero_snr=True, timestep_spacing="trailing")
@@ -95,7 +96,7 @@ def synthetic_inputs(frames: int, size: int, seed: int = 0, noise_bk: bool = Fal
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -133,13 +134,23 @@ def measured_peaks():
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         d = json.loads(p.read_text())
-        return d.get("bf16_tflops_sustained", 1439.7), d.get("hbm_gbs", 6566.4), "measured (MEASURED_PEAKS.json, sustained)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json, sustained)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense fp16/bf16, HBM3 at 700 W), not a measured rate"
 
 
 # =====================================================================================================
 # our engine
 # =====================================================================================================
+def dump_outputs(out: dict, directory: str) -> None:
+    """What sample_tensors() returned in the last timed step, as float32 .npy files: `latents` whole, `videos` (the
+    decoded clip, 75 MB in fp32 at the default config) on every second pixel in both directions, so the files stay
+    well under 64 MB together."""
+    d = Path(directory)
+    d.mkdir(parents=True, exist_ok=True)
+    np.save(d / "latents.npy", out["latents"].float().cpu().numpy())
+    np.save(d / "videos.npy", out["videos"][..., ::2, ::2].float().cpu().numpy())
+
+
 def build_pipeline(device, rank: int = 0, world: int = 1):
     from transformers import CLIPVisionConfig, CLIPVisionModelWithProjection
 
@@ -217,6 +228,8 @@ def run_ours(args):
     sync()
     ms = e0.elapsed_time(e1)
     launches = ops.launches() - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(out, args.dump_outputs)
     clocks = sampler.stop() if rank == 0 else None
     pipe._collect_timings()
     phases = dict(pipe.timings)
@@ -286,9 +299,9 @@ def run_ours(args):
             for name, (t_ms, fl, by, cnt) in sorted(agg.items(), key=lambda kv: -kv[1][0]):
                 calls[name] = {"ms": round(t_ms, 2), "launches": cnt, "tflops": round(fl / t_ms / 1e9, 1) if fl else None,
                                "gbs": round(by / t_ms / 1e6, 1)}
-            # The dominant kernel is gemm_tcgen05_kernel: the plain GEMMs ("gemm") and the implicit-GEMM 3x3 convolutions
+            # The dominant kernel is gemm_wgmma_kernel: the plain GEMMs ("gemm") and the implicit-GEMM 3x3 convolutions
             # ("conv3x3") are the same kernel template in its two addressing modes.
-            fam = {"gemm_tcgen05_kernel": ("gemm", "conv3x3"), "attn_spatial": ("attn_spatial",)}
+            fam = {"gemm_wgmma_kernel": ("gemm", "conv3x3"), "attn_spatial": ("attn_spatial",)}
             fam_ms = {k: sum(agg[n][0] for n in names if n in agg) for k, names in fam.items()}
             others = {n: agg[n][0] for n in agg if not any(n in names for names in fam.values())}
             dname = max({**fam_ms, **others}.items(), key=lambda kv: kv[1])[0]
@@ -297,10 +310,10 @@ def run_ours(args):
             dfl = sum(agg[n][1] for n in members if n in agg)
             dby = sum(agg[n][2] for n in members if n in agg)
             dcnt = sum(agg[n][3] for n in members if n in agg)
-            tensor_bound = dname in ("gemm_tcgen05_kernel", "attn_spatial")
+            tensor_bound = dname in ("gemm_wgmma_kernel", "attn_spatial")
             achieved = dfl / dms / 1e9 if tensor_bound else dby / dms / 1e6
             peak = peak_tf if tensor_bound else peak_gbs
-            # DRAM bytes per launch of this kernel from the committed `ncu --set full` capture of THIS gpu count, else null
+            # DRAM bytes per launch of this kernel from a committed `ncu --set full` capture of THIS gpu count, else null
             traffic, traffic_src = None, None
             tpath = ROOT / "profiles" / "ncu_traffic.json"
             if tpath.exists():
@@ -547,12 +560,18 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", type=int, default=2, help="BASELINE.json config number: 2 (default, the metric), 4, 5")
     ap.add_argument("--dump-calls", default=None, help="write every profiled C-ABI call (name, flops, bytes, ms) as CSV")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs to DIR/latents.npy and DIR/videos.npy (float32)")
     ap.add_argument("--no-cpu-baseline", action="store_true", help="skip the CPU sample (development runs)")
     ap.add_argument("--no-breakdown", action="store_true",
                     help="skip the two extra diagnostic clips (event-bracketed calls, CUPTI table): roofline = null")
     ap.add_argument("--one-clip", action="store_true",
-                    help="run exactly one device-resident clip and exit (for `ncu` launch lists; not a bench value)")
+                    help="run exactly one device-resident clip and exit (a profiling aid; not a bench value)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.impl == "reference" or args.one_clip):
+        ap.error("--dump-outputs writes the timed steps' outputs of the engine: not with --impl reference or --one-clip")
     select_config(args.config)
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-/* mimo_b200 — C ABI of the B200 (sm_100a) denoising-engine kernels.
+/* mimo_b200 — C ABI of the H100 (sm_90a) denoising-engine kernels.
  *
  * The reference (menyifang/MIMO) has no FFI layer: every op on its hot path is a PyTorch library call made
  * from src/models/*.py. Each entry point below replaces one of those call sites (cited per function as
@@ -11,7 +11,7 @@
  *    allocate: all entry points are CUDA-graph capturable.
  *  - dtype: 0 = fp16, 1 = bf16 storage; accumulation and all epilogue math are fp32.
  *  - return 0 on success, negative on error; mimo_last_error() gives the thread-local message.
- *  - there is no CPU fallback: on a machine without an sm_100 device every compute entry point fails.
+ *  - there is no CPU fallback: on a machine without an sm_90 device every compute entry point fails.
  */
 #ifndef MIMO_B200_H_
 #define MIMO_B200_H_
@@ -38,7 +38,7 @@ extern "C" {
 
 const char* mimo_version(void);
 const char* mimo_last_error(void);
-/* 0 if device `dev` is sm_100; MIMO_ERR_DEVICE otherwise (also when there is no CUDA device at all). */
+/* 0 if device `dev` is sm_90; MIMO_ERR_DEVICE otherwise (also when there is no CUDA device at all). */
 int mimo_device_check(int dev);
 /* sizeof() of the parameter structs as compiled into the library (0 epilogue, 1 gemm, 2 conv3x3, 3 groupnorm,
  * 4 attn, 5 attn_temporal, 6 exchange): lets a binding verify its struct mirrors before the first call. */
@@ -57,7 +57,7 @@ typedef struct {
   int act;     /* MIMO_ACT_*                                                               */
 } mimo_epilogue;
 
-/* out[M,N] = epilogue(A[M,K] . W[N,K]^T).  tcgen05 GEMM, TMA-fed, fp32 accumulate in TMEM.
+/* out[M,N] = epilogue(A[M,K] . W[N,K]^T).  wgmma GEMM, TMA-fed, fp32 accumulate in registers.
  * Replaces: torch.nn.Linear / 1x1 Conv2d call sites — to_q/k/v/to_out (diffusers Attention, constructed at
  * src/models/attention.py:321-345, src/models/motion_module.py:282-292), FeedForward/GEGLU
  * (src/models/attention.py:359, motion_module.py:235), proj_in/proj_out (src/models/transformer_3d.py:64-66,
@@ -78,8 +78,8 @@ typedef struct {
   mimo_epilogue ep;
   /* optional scratch (device, 16-byte aligned, contents irrelevant, may be shared by all calls of a stream): lets small-M /
    * long-K problems split the K loop over several CTAs (fp32 partials, summed in a fixed order by a second kernel:
-   * deterministic). NULL = never split. (Disabled by default inside the library: measured slower on B200 at the shapes
-   * of this path - see csrc/gemm_tcgen05.cu.) */
+   * deterministic). NULL = never split. (Disabled by default inside the library - see
+   * csrc/gemm_wgmma.cu.) */
   void* workspace;
   int64_t workspace_bytes;
 } mimo_gemm_params;
@@ -156,7 +156,7 @@ int mimo_layernorm(const void* x, const void* gamma, const void* beta, void* out
                    float eps, const void* pe, int64_t rows_per_frame, int32_t frames, int32_t pe_frame_offset,
                    int32_t dtype, void* stream);
 
-/* Spatial self-attention with the reference-image bank (flash attention, tcgen05 QK^T and PV, online softmax).
+/* Spatial self-attention with the reference-image bank (flash attention, wgmma QK^T and PV, online softmax).
  * q/k/v: [n, lq, heads, d] slices of a fused QKV buffer (row stride ld_qkv elements). bank_k/bank_v:
  * [nb, lb, heads, d] with row stride ld_bank; frame-sample i attends to [self keys | bank keys of branch
  * bank_index[i]] when bank_index[i] >= 0, and to self keys only when bank_index[i] < 0 (the unconditional half).

@@ -1,4 +1,4 @@
-"""Build the sm_100a C-ABI library in-tree (mimo_b200/libmimo_b200.so) with nvcc.
+"""Build the sm_90a C-ABI library in-tree (mimo_b200/libmimo_b200.so) with nvcc.
 
 No torch types cross the boundary, so this is a plain `nvcc -shared` of the .cu files under csrc/; cudart is
 linked statically and the driver (for cuTensorMapEncodeTiled) is resolved at run time, so the library loads
@@ -20,7 +20,7 @@ LIB = PKG / "libmimo_b200.so"
 OBJ = PKG / "build"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "-Xptxas=-v",
@@ -38,10 +38,13 @@ def _sources():
     return sorted(CSRC.glob("*.cu"))
 
 
+GEN_WGMMA = PKG.parent / "scripts" / "gen_wgmma.py"  # writes wgmma.cuh (one wrapper per wgmma shape) into OBJ
+
+
 def _digest() -> str:
     h = hashlib.sha256()
     for p in sorted(list(CSRC.glob("*.cu")) + list(CSRC.glob("*.cuh")) + list(CSRC.glob("*.h"))
-                    + [PKG.parent / "include" / "mimo_b200.h"]):
+                    + [PKG.parent / "include" / "mimo_b200.h", GEN_WGMMA]):
         h.update(p.name.encode())
         h.update(p.read_bytes())
     h.update(" ".join(NVCC_FLAGS).encode())
@@ -54,11 +57,14 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     if not force and LIB.exists() and stamp.exists() and stamp.read_text() == dig:
         return LIB
     OBJ.mkdir(exist_ok=True)
+    r = subprocess.run([sys.executable, str(GEN_WGMMA), str(OBJ / "wgmma.cuh")], capture_output=True, text=True)
+    if r.returncode != 0:
+        raise RuntimeError(f"gen_wgmma.py failed:\n{r.stdout}\n{r.stderr}")
     nvcc = _nvcc()
 
     def compile_one(src: Path) -> Path:
         obj = OBJ / (src.stem + ".o")
-        cmd = [nvcc, *NVCC_FLAGS, "-c", str(src), "-o", str(obj)]
+        cmd = [nvcc, *NVCC_FLAGS, "-I", str(OBJ), "-c", str(src), "-o", str(obj)]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"nvcc failed for {src.name}:\n{r.stdout}\n{r.stderr}")

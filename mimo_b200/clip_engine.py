@@ -4,7 +4,7 @@ The reference calls `self.image_encoder(clip_image).image_embeds` once per clip 
 transformers.CLIPVisionModelWithProjection (pipeline_pose2vid_long_edit_bkfill_roiclip.py:378-385; the module is built at
 run_animate.py:92-94). The caller still passes that module; only its state dict and config are read here, and the
 forward runs as C-ABI kernel calls: patch embedding as one GEMM over unfolded 14x14 patches, then per layer
-LN -> fused q|k|v GEMM (+bias) -> flash attention (tcgen05, d = 64) -> out-proj GEMM (+bias, +residual) -> LN ->
+LN -> fused q|k|v GEMM (+bias) -> flash attention (wgmma, d = 64) -> out-proj GEMM (+bias, +residual) -> LN ->
 fc1 GEMM (+bias) -> quick-GELU -> fc2 GEMM (+bias, +residual); pooled = post-LN of the class token; projection GEMM.
 """
 from __future__ import annotations

@@ -1,58 +1,62 @@
-// Spatial self-attention with the reference-image bank: flash attention on tcgen05.
+// Spatial self-attention with the reference-image bank: flash attention on wgmma.
 //
-// One CTA = 128 query rows of one (frame-sample n, head h). The key/value sequence is [self tokens | bank
-// tokens of branch bank_index[n]] (bank skipped when bank_index[n] < 0: the unconditional CFG half attends to
-// itself only, which is what src/models/mutual_self_attention.py:177-197 computes by running attn1 a second
-// time). Per 128-key tile:
-//     S  = Q K^T         tcgen05.mma 128x128x(d rounded to 16), Q and K tiles K-major, fp32 S in TMEM
-//     P  = exp2(S*c - m) softmax warps: one thread per query row (TMEM lane), online max / sum in fp32,
-//                        P written to shared memory as the 128B-swizzled K-major A operand
-//     O += P V           tcgen05.mma 128x(d rounded to 16)x128, V tile used as an MN-major B operand
+// One CTA = 128 query rows (64 from d = 160 on, see AttnCfg) of one (frame-sample n, head h). The key/value sequence
+// is [self tokens | bank tokens of branch bank_index[n]] (bank skipped when bank_index[n] < 0: the unconditional CFG
+// half attends to itself only, which is what src/models/mutual_self_attention.py:177-197 computes by running attn1 a
+// second time). Roles: each MMA warpgroup owns 64 query rows and, per 128-key tile:
+//     S  = Q K^T         wgmma m64n128k16 (d rounded to 16 / 16 steps), Q and K tiles K-major, fp32 S in registers
+//     P  = exp2(S*c - m) online max / sum in fp32 (a row lives in the 4 lanes of a quad), P converted in registers to
+//                        the A fragments of the next MMA - it never touches shared memory
+//     O += P V           wgmma m64n(d rounded to 16)k16, A = P from registers, V tile as an MN-major B operand
+// and one thread of the warp after the MMA warpgroups issues the TMA loads.
 // Q/K/V tiles arrive by 4-D TMA boxes straight out of the fused QKV activation buffer ([token, 3C] rows, head
 // slices addressed by a tensor-map dimension); head dims 40/80/160 are zero-filled up to 64-element chunks by
 // TMA's out-of-bounds handling, so no padded copies exist in HBM.
-// Roles: warp 0 lane 0 TMA, warp 1 lane 0 MMA, warp 2 TMEM alloc, warps 4-7 softmax/correction/epilogue.
 #include <cuda_runtime.h>
 
 #include "../../include/mimo_b200.h"
 #include "attn_common.h"
 #include "host_util.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace mimo {
 
-constexpr int kAttnThreads = 256;
-static int g_attn_variant = 0;  // test hook: 0 = auto, 1 = force the single-tile kernel
-
-template <int NCH, int KVST>
+// Registers are reserved per group of 4 warps. With two MMA warpgroups (+ the TMA warp = 12 warps' worth) a thread may
+// hold 168 registers: enough for S (64) + O (d/2) below d = 160. From d = 160 on a CTA has ONE MMA warpgroup (64 query
+// rows, 8 warps' worth, up to 255 registers), so O, S and P stay in registers without spills, and the smaller Q tile
+// leaves room for a second K/V stage.
+template <int DP>
 struct AttnCfg {
-  static constexpr int kQBytes = NCH * kChunkBytes;
+  static constexpr int NCH = (DP + 63) / 64;                   // 64-column chunks of Q / K / V
+  static constexpr int NWG = DP >= 160 ? 1 : 2;                // MMA warpgroups, 64 query rows each
+  static constexpr int QROWS = 64 * NWG;                       // query rows per CTA
+  static constexpr int kThreads = 128 * NWG + 32;              // + the TMA warp (warp 4 * NWG)
+  static constexpr int kQChunk = QROWS * 128;                  // one 64-column chunk of the Q tile
+  static constexpr int kQBytes = NCH * kQChunk;
   static constexpr int kKVStageBytes = 2 * NCH * kChunkBytes;  // K chunks then V chunks
-  static constexpr int kPBytes = 2 * kChunkBytes;
-  static constexpr int kSmemBytes = kQBytes + KVST * kKVStageBytes + kPBytes + 1024 + 256;
-  static constexpr int kTmemCols = (NCH <= 2) ? 256 : 512;
+  static constexpr int kFit = (227 * 1024 - 1024 - 256 - kQBytes) / kKVStageBytes;
+  static constexpr int KVST = kFit < 3 ? kFit : 3;             // K/V stages that fit next to Q
+  static constexpr int kSmemBytes = kQBytes + KVST * kKVStageBytes + 1024 + 256;
+  static_assert(KVST >= 1, "K/V tile does not fit");
 };
 
-template <int NCH, int KVST, bool kBf16>
-__global__ void __launch_bounds__(kAttnThreads)
+template <int DP, bool kBf16>
+__global__ void __launch_bounds__(AttnCfg<DP>::kThreads, 1)
 attn_spatial_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmBK,
                     const __grid_constant__ CUtensorMap tmBV, AttnArgs a) {
-  using Cfg = AttnCfg<NCH, KVST>;
+  using Cfg = AttnCfg<DP>;
   using C = Cvt<kBf16>;
+  constexpr int NCH = Cfg::NCH, KVST = Cfg::KVST, kProd = 4 * Cfg::NWG;  // kProd: the TMA warp
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
   uint8_t* sKV = sQ + Cfg::kQBytes;
-  uint8_t* sP = sKV + KVST * Cfg::kKVStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + Cfg::kPBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + KVST * Cfg::kKVStageBytes);
   uint64_t* q_full = bars;
   uint64_t* kv_full = bars + 1;
   uint64_t* kv_empty = kv_full + KVST;
-  uint64_t* s_full = kv_empty + KVST;
-  uint64_t* p_full = s_full + 1;
-  uint64_t* o_done = p_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_done + 1);
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);  // provably warp-uniform for the compiler
   const int lane = threadIdx.x & 31;
@@ -64,7 +68,7 @@ attn_spatial_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   const int bidx = __shfl_sync(0xffffffffu, a.bank_index ? a.bank_index[n] : -1, 0);
   const int T = a.n_self_tiles + (bidx >= 0 ? a.n_bank_tiles : 0);
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kProd && lane == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
@@ -73,30 +77,21 @@ attn_spatial_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       tma_prefetch_desc(&tmBV);
     }
   }
-  if (warp == 1 && lane == 0) {
+  if (warp == kProd && lane == 1) {
     mbar_init(q_full, 1);
     for (int s = 0; s < KVST; ++s) {
       mbar_init(&kv_full[s], 1);
-      mbar_init(&kv_empty[s], 1);
+      mbar_init(&kv_empty[s], kProd);  // lane 0 of each MMA warp, once its P.V has read the stage
     }
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 128);
-    mbar_init(o_done, 1);
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, Cfg::kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
-  const uint32_t tmem_S = tmem_base;        // 128 fp32 columns
-  const uint32_t tmem_O = tmem_base + 128;  // dp fp32 columns
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kProd && lane == 0) {
     // ===================== TMA producer =====================
     mbar_expect_tx(q_full, Cfg::kQBytes);
 #pragma unroll
-    for (int ch = 0; ch < NCH; ++ch) tma_load_4d(sQ + ch * kChunkBytes, &tmQ, q_full, ch * 64, h, q_tile * BQ, n);
+    for (int ch = 0; ch < NCH; ++ch) tma_load_4d(sQ + ch * Cfg::kQChunk, &tmQ, q_full, ch * 64, h, q_tile * Cfg::QROWS, n);
     for (int j = 0; j < T; ++j) {
       const int stage = j % KVST;
       const uint32_t phase = (j / KVST) & 1u;
@@ -115,208 +110,149 @@ attn_spatial_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         tma_load_4d(sv + ch * kChunkBytes, mv, &kv_full[stage], ch * 64, h, row0, img);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (whole warp, one elected lane issues: descriptors stay uniform) =====================
-    const uint32_t idesc_qk = make_idesc_f16(BQ, BKV, kBf16, false, false);
-    const uint32_t idesc_pv = make_idesc_f16(BQ, a.dp, kBf16, false, true);  // B (= V) is MN-major
-    const int ksteps_qk = a.dp / 16;
-    const uint32_t q_addr = smem_u32(sQ);
-    const uint32_t p_addr = smem_u32(sP);
-    auto issue_qk = [&](int j) {
-      const int stage = j % KVST;
-      const uint32_t k_addr = smem_u32(sKV + stage * Cfg::kKVStageBytes);
-      if (elect_one()) {
-        for (int ks = 0; ks < ksteps_qk; ++ks) {
-          const uint32_t off = (ks >> 2) * kChunkBytes + (ks & 3) * 32;
-          umma_ss(tmem_S, make_smem_desc_sw128(q_addr + off, 16, 1024), make_smem_desc_sw128(k_addr + off, 16, 1024),
-                  idesc_qk, ks != 0 ? 1u : 0u);
-        }
-        tc_commit(s_full);
-      }
-      __syncwarp();
-    };
+  } else if (warp < kProd) {
+    // ===================== MMA / softmax / epilogue =====================
+    const int wg = warp >> 2;  // query rows [64 wg, 64 wg + 64) of the tile
+    // accumulator layout (S and O alike): this thread holds rows rbase and rbase + 8; fragment j (8 columns) holds
+    // columns 8 j + q2, + 1 in [4 j], [4 j + 1] (row rbase) and [4 j + 2], [4 j + 3] (row rbase + 8)
+    const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int q2 = (lane & 3) * 2;
+    const uint32_t q_addr = smem_u32(sQ) + wg * (64 * 128);
+    float o[DP / 2];
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
     mbar_wait(q_full, 0);
-    mbar_wait(&kv_full[0], 0);
-    tc_fence_after();
-    issue_qk(0);
     for (int j = 0; j < T; ++j) {
       const int stage = j % KVST;
-      mbar_wait(p_full, j & 1);
-      tc_fence_after();
-      const uint32_t v_addr = smem_u32(sKV + stage * Cfg::kKVStageBytes + NCH * kChunkBytes);
-      if (elect_one()) {
-#pragma unroll
-        for (int ks = 0; ks < BKV / 16; ++ks) {
-          // A = P: K-major, 64-key chunks of [128 rows x 128 B]; B = V: MN-major, 16 keys = 2 KiB further down
-          const uint32_t pa = p_addr + (ks >> 2) * kChunkBytes + (ks & 3) * 32;
-          const uint32_t vb = v_addr + ks * 2048;
-          umma_ss(tmem_O, make_smem_desc_sw128(pa, 16, 1024), make_smem_desc_sw128(vb, kChunkBytes, 1024), idesc_pv,
-                  (j | ks) != 0 ? 1u : 0u);
-        }
-        tc_commit(&kv_empty[stage]);
-        tc_commit(o_done);
-      }
-      __syncwarp();
-      if (j + 1 < T) {
-        const int ns = (j + 1) % KVST;
-        mbar_wait(&kv_full[ns], ((j + 1) / KVST) & 1u);
-        tc_fence_after();
-        issue_qk(j + 1);
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== softmax / correction / epilogue =====================
-    const int ew = warp & 3;
-    const int r = ew * 32 + lane;  // query row inside the tile == TMEM lane
-    const uint32_t lane_off = static_cast<uint32_t>(ew * 32) << 16;
-    float m = -INFINITY, l = 0.f;
-    uint8_t* prow = sP + r * 128;
-    const int sw = r & 7;
-    for (int j = 0; j < T; ++j) {
       const bool bank = j >= a.n_self_tiles;
       const int len = bank ? a.lb : a.lq;
       const int row0 = (bank ? j - a.n_self_tiles : j) * BKV;
       int valid = len - row0;
       if (valid > BKV) valid = BKV;
-      mbar_wait(s_full, j & 1);
-      tc_fence_after();
-      // pass 1: row maximum
-      float mx = -INFINITY;
+      mbar_wait(&kv_full[stage], (j / KVST) & 1u);
+      const uint32_t k_addr = smem_u32(sKV + stage * Cfg::kKVStageBytes);
+      const uint32_t v_addr = k_addr + NCH * kChunkBytes;
+
+      float s[BKV / 2];
+      wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t v[32];
-        tmem_ld_x32(tmem_S + lane_off + c * 32, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i)
-          if (c * 32 + i < valid) mx = fmaxf(mx, __uint_as_float(v[i]));
+      for (int ks = 0; ks < DP / 16; ++ks) {
+        const uint32_t off = (ks & 3) * 32;
+        Wgmma<BKV, kBf16>::ss(s, make_smem_desc_sw128(q_addr + (ks >> 2) * Cfg::kQChunk + off, 16, 1024),
+                              make_smem_desc_sw128(k_addr + (ks >> 2) * kChunkBytes + off, 16, 1024), ks != 0 ? 1u : 0u);
       }
-      const float m_new = fmaxf(m, mx * a.scale_log2);
-      const float alpha = exp2f(m - m_new);
-      // P (and O) may only be overwritten once the previous P.V has retired
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(s);
+
+      // row maximum over the valid keys (a row is spread over the 4 lanes of a quad)
+      float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int jn = 0; jn < BKV / 8; ++jn)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          if (8 * jn + q2 + (e & 1) < valid)
+            mx[e >> 1] = fmaxf(mx[e >> 1], s[4 * jn + e]);
+          else
+            s[4 * jn + e] = -INFINITY;
+        }
+      float alpha[2], m_new[2];
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+        m_new[r] = fmaxf(m[r], mx[r] * a.scale_log2);
+        alpha[r] = exp2f(m[r] - m_new[r]);
+      }
+      // probabilities -> A fragments of P.V: k-step kk covers keys [16 kk, 16 kk + 16) = S fragments 2 kk, 2 kk + 1
+      uint32_t pa[BKV / 16][4];
+      float rowsum[2] = {0.f, 0.f};
+#pragma unroll
+      for (int kk = 0; kk < BKV / 16; ++kk)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int e = 8 * kk + 2 * i;  // i: (row, keys 0-7), (row + 8, keys 0-7), (row, keys 8-15), (row + 8, keys 8-15)
+          const int r = i & 1;
+          const float p0 = exp2f(fmaf(s[e], a.scale_log2, -m_new[r]));
+          const float p1 = exp2f(fmaf(s[e + 1], a.scale_log2, -m_new[r]));
+          rowsum[r] += p0 + p1;
+          pa[kk][i] = C::pack(p0, p1);
+        }
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        l[r] = l[r] * alpha[r] + rowsum[r];
+        m[r] = m_new[r];
+      }
       if (j > 0) {
-        mbar_wait(o_done, (j - 1) & 1);
-        tc_fence_after();
+#pragma unroll
+        for (int i = 0; i < DP / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
       }
-      // pass 2: probabilities -> swizzled smem (A operand of P.V)
-      float rowsum = 0.f;
+      wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t v[32];
-        tmem_ld_x32(tmem_S + lane_off + c * 32, v);
-        tmem_ld_wait();
-        uint32_t pk[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int c0 = c * 32 + 2 * i;
-          float p0 = 0.f, p1 = 0.f;
-          if (c0 < valid) p0 = exp2f(fmaf(__uint_as_float(v[2 * i]), a.scale_log2, -m_new));
-          if (c0 + 1 < valid) p1 = exp2f(fmaf(__uint_as_float(v[2 * i + 1]), a.scale_log2, -m_new));
-          rowsum += p0 + p1;
-          pk[i] = C::pack(p0, p1);
-        }
-        // 32 keys = 64 B = four 16-byte pieces of this row's 128-B line in chunk (c >> 1)
-        uint8_t* line = prow + (c >> 1) * kChunkBytes;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int piece = (c & 1) * 4 + q;
-          *reinterpret_cast<uint4*>(line + ((piece ^ sw) << 4)) =
-              make_uint4(pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
-        }
+      for (int kk = 0; kk < BKV / 16; ++kk) {
+        // B = V: MN-major, 16 keys = 2 KiB further down; 64-column chunks kChunkBytes apart
+        Wgmma<DP, kBf16>::rs(o, pa[kk], make_smem_desc_sw128(v_addr + kk * 2048, kChunkBytes, 1024),
+                             (j | kk) != 0 ? 1u : 0u);
       }
-      l = l * alpha + rowsum;
-      m = m_new;
-      // correction: O *= alpha
-      if (j > 0) {
-        for (int c = 0; c < a.dp / 16; ++c) {
-          uint32_t v[16];
-          tmem_ld_x16(tmem_O + lane_off + c * 16, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * alpha);
-          tmem_st_x16(tmem_O + lane_off + c * 16, v);
-        }
-        tmem_st_wait();
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(p_full);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(o);
+      if (lane == 0) mbar_arrive(&kv_empty[stage]);
     }
     // epilogue: O / l -> global
-    mbar_wait(o_done, (T - 1) & 1);
-    tc_fence_after();
-    const float inv_l = 1.0f / l;
-    const int qrow = q_tile * BQ + r;
-    typename C::T* orow =
-        static_cast<typename C::T*>(a.out) + (static_cast<long long>(n) * a.lq + qrow) * a.ld_out + h * a.d;
-    for (int c = 0; c < a.dp / 16; ++c) {
-      uint32_t v[16];
-      tmem_ld_x16(tmem_O + lane_off + c * 16, v);
-      tmem_ld_wait();
-      if (qrow < a.lq) {
 #pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          if (c * 16 + q * 8 < a.d) {
-            uint4 o;
-            o.x = C::pack(__uint_as_float(v[q * 8 + 0]) * inv_l, __uint_as_float(v[q * 8 + 1]) * inv_l);
-            o.y = C::pack(__uint_as_float(v[q * 8 + 2]) * inv_l, __uint_as_float(v[q * 8 + 3]) * inv_l);
-            o.z = C::pack(__uint_as_float(v[q * 8 + 4]) * inv_l, __uint_as_float(v[q * 8 + 5]) * inv_l);
-            o.w = C::pack(__uint_as_float(v[q * 8 + 6]) * inv_l, __uint_as_float(v[q * 8 + 7]) * inv_l);
-            *reinterpret_cast<uint4*>(orow + c * 16 + q * 8) = o;
-          }
-        }
+    for (int r = 0; r < 2; ++r) {
+      l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
+      l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
+      const float inv_l = 1.0f / l[r];
+      const int qrow = q_tile * Cfg::QROWS + rbase + 8 * r;
+      if (qrow < a.lq) {
+        typename C::T* orow =
+            static_cast<typename C::T*>(a.out) + (static_cast<long long>(n) * a.lq + qrow) * a.ld_out + h * a.d;
+#pragma unroll
+        for (int jn = 0; jn < DP / 8; ++jn)
+          if (8 * jn + q2 < a.d)
+            *reinterpret_cast<uint32_t*>(orow + 8 * jn + q2) = C::pack(o[4 * jn + 2 * r] * inv_l, o[4 * jn + 2 * r + 1] * inv_l);
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
   }
 }
 
-template <int NCH, int KVST, bool kBf16>
-static int launch_attn(const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v, const CUtensorMap& bk,
-                       const CUtensorMap& bv, const AttnArgs& a, dim3 grid, cudaStream_t st) {
-  using Cfg = AttnCfg<NCH, KVST>;
-  auto kern = attn_spatial_kernel<NCH, KVST, kBf16>;
+static int attn_tmap(CUtensorMap* m, int dtype, const void* base, int d, int heads, int len, int nimg, long long ld,
+                     uint32_t rows = BKV);
+
+template <int DP, bool kBf16>
+static int launch_attn(const mimo_attn_params* p, const CUtensorMap& k, const CUtensorMap& v, const CUtensorMap& bk,
+                       const CUtensorMap& bv, const AttnArgs& a, cudaStream_t st) {
+  using Cfg = AttnCfg<DP>;
+  auto kern = attn_spatial_kernel<DP, kBf16>;
   static bool attr_done = false;
   if (!attr_done) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e != cudaSuccess) return set_cuda_error("cudaFuncSetAttribute(attn)", e);
     attr_done = true;
   }
-  cudaError_t e = launch_k(kern, grid, dim3(kAttnThreads), Cfg::kSmemBytes, st, q, k, v, bk, bv, a);
+  CUtensorMap q;  // Q boxes cover the CTA's query rows
+  if (int rc = attn_tmap(&q, p->dtype, p->q, p->d, p->heads, p->lq, p->n, p->ld_qkv, Cfg::QROWS)) return rc;
+  const dim3 grid((p->lq + Cfg::QROWS - 1) / Cfg::QROWS, p->heads, p->n);
+  cudaError_t e = launch_k(kern, grid, dim3(Cfg::kThreads), Cfg::kSmemBytes, st, q, k, v, bk, bv, a);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) return set_cuda_error("attn launch", e);
   return MIMO_OK;
 }
 
-static int attn_tmap(CUtensorMap* m, int dtype, const void* base, int d, int heads, int len, int nimg,
-                     long long ld) {
+static int attn_tmap(CUtensorMap* m, int dtype, const void* base, int d, int heads, int len, int nimg, long long ld,
+                     uint32_t rows) {
   const uint64_t dims[4] = {static_cast<uint64_t>(d), static_cast<uint64_t>(heads), static_cast<uint64_t>(len),
                             static_cast<uint64_t>(nimg)};
   const uint64_t str[3] = {static_cast<uint64_t>(d) * 2, static_cast<uint64_t>(ld) * 2,
                            static_cast<uint64_t>(len) * ld * 2};
-  const uint32_t box[4] = {64, 1, 128, 1};
+  const uint32_t box[4] = {64, 1, rows, 1};
   return encode_tmap(m, dtype, 4, base, dims, str, box);
 }
 
 }  // namespace mimo
 
 using namespace mimo;
-
-extern "C" int mimo_debug_attn_variant(int v) {
-  g_attn_variant = v;
-  return 0;
-}
-static long long* g_attn_trace = nullptr;
-extern "C" int mimo_debug_attn_trace(void* buf) {  // >= 5120 int64 of device memory, or NULL
-  g_attn_trace = static_cast<long long*>(buf);
-  return 0;
-}
 
 extern "C" int mimo_attn_spatial(const mimo_attn_params* p, void* stream) {
   if (!p || !p->q || !p->k || !p->v || !p->out) return set_error(MIMO_ERR_ARG, "mimo_attn_spatial: null pointer");
@@ -329,8 +265,6 @@ extern "C" int mimo_attn_spatial(const mimo_attn_params* p, void* stream) {
 
   AttnArgs a;
   a.lq = p->lq;
-  a.variant = g_attn_variant;
-  a.trace = g_attn_trace;
   a.lb = has_bank ? p->lb : 0;
   a.heads = p->heads;
   a.d = p->d;
@@ -342,8 +276,7 @@ extern "C" int mimo_attn_spatial(const mimo_attn_params* p, void* stream) {
   a.out = p->out;
   a.ld_out = p->ld_out;
 
-  CUtensorMap tq, tk, tv, tbk, tbv;
-  if (int rc = attn_tmap(&tq, p->dtype, p->q, p->d, p->heads, p->lq, p->n, p->ld_qkv)) return rc;
+  CUtensorMap tk, tv, tbk, tbv;
   if (int rc = attn_tmap(&tk, p->dtype, p->k, p->d, p->heads, p->lq, p->n, p->ld_qkv)) return rc;
   if (int rc = attn_tmap(&tv, p->dtype, p->v, p->d, p->heads, p->lq, p->n, p->ld_qkv)) return rc;
   if (has_bank) {
@@ -354,19 +287,16 @@ extern "C" int mimo_attn_spatial(const mimo_attn_params* p, void* stream) {
     tbk = tk;
     tbv = tv;
   }
-  dim3 grid((p->lq + BQ - 1) / BQ, p->heads, p->n);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int nch = (a.dp + 63) / 64;
-  const bool bf = p->dtype == MIMO_BF16;
-  // d + 1 <= 64 (the 64x64 level, d = 40: MUFU-bound): two softmax threads per row + row sum on the tensor pipe
-  // (attn_spatial_pp2.cu; measured 467 vs 429 TFLOP/s). Variant bit 16 forces it wherever it applies, bit 32 disables it.
-  if (attn_pp2_supports(p->d) && !(g_attn_variant & 32) && g_attn_variant != 1 && ((g_attn_variant & 16) || p->d + 1 <= 64))
-    return launch_attn_pp2(bf, tq, tk, tv, tbk, tbv, a, p->n, st);
-  if (nch <= 2 && g_attn_variant != 1) return launch_attn_pp(bf, tq, tk, tv, tbk, tbv, a, p->n, st);
-  if (nch == 1) return bf ? launch_attn<1, 2, true>(tq, tk, tv, tbk, tbv, a, grid, st)
-                          : launch_attn<1, 2, false>(tq, tk, tv, tbk, tbv, a, grid, st);
-  if (nch == 2) return bf ? launch_attn<2, 2, true>(tq, tk, tv, tbk, tbv, a, grid, st)
-                          : launch_attn<2, 2, false>(tq, tk, tv, tbk, tbv, a, grid, st);
-  return bf ? launch_attn<3, 1, true>(tq, tk, tv, tbk, tbv, a, grid, st)
-            : launch_attn<3, 1, false>(tq, tk, tv, tbk, tbv, a, grid, st);
+  // one instantiation per head dim rounded up to 16 (the P.V instruction's N)
+  switch (a.dp) {
+#define MIMO_ATTN_DP(DP) \
+  case DP:               \
+    return p->dtype == MIMO_BF16 ? launch_attn<DP, true>(p, tk, tv, tbk, tbv, a, st) \
+                                 : launch_attn<DP, false>(p, tk, tv, tbk, tbv, a, st);
+    MIMO_ATTN_DP(16) MIMO_ATTN_DP(32) MIMO_ATTN_DP(48) MIMO_ATTN_DP(64) MIMO_ATTN_DP(80) MIMO_ATTN_DP(96)
+    MIMO_ATTN_DP(112) MIMO_ATTN_DP(128) MIMO_ATTN_DP(144) MIMO_ATTN_DP(160) MIMO_ATTN_DP(176) MIMO_ATTN_DP(192)
+#undef MIMO_ATTN_DP
+  }
+  return set_error(MIMO_ERR_ARG, "mimo_attn_spatial: unsupported head dim");
 }

@@ -5,7 +5,7 @@
 // organised around memory: one CTA stages the Q, K and V rows of all frames of one pixel (for a group of heads) in
 // shared memory with 128-bit loads — every row is a contiguous C-element segment, so the reference's
 // "(b f) d c <-> (b d) f c" transposes never materialise — and one warp per head then runs the attention on tensor
-// cores with warp-level mma.sync.m16n8k16 (a 24-row problem cannot fill a 128-row tcgen05 tile): S = Q K^T from
+// cores with warp-level mma.sync.m16n8k16 (a 24-row problem cannot fill a 64-row wgmma tile): S = Q K^T from
 // ldmatrix fragments, fp32 softmax in the accumulator registers, P re-used in registers as the A operand of P V,
 // V read with ldmatrix.trans. Outputs are staged through shared memory for 128-bit stores.
 //

@@ -20,7 +20,7 @@ int set_cuda_error(const char* what, cudaError_t e) {
 }
 
 static int g_dev_state = 0;  // 0 unknown, 1 ok, -1 bad
-static int g_num_sms = 148;
+static int g_num_sms = 132;
 
 int ensure_device() {
   if (g_dev_state == 1) return MIMO_OK;
@@ -34,19 +34,19 @@ int ensure_device() {
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (major != 10) {
-    snprintf(g_err, sizeof(g_err), "device %d is sm_%d%d; mimo_b200 kernels are built for sm_100a only", dev,
+  if (major != 9 || minor != 0) {  // sm_90a code (wgmma, setmaxnreg) loads on compute capability 9.0 only
+    snprintf(g_err, sizeof(g_err), "device %d is sm_%d%d; mimo_b200 kernels are built for sm_90a only", dev,
              major, minor);
     g_dev_state = -1;
     return MIMO_ERR_DEVICE;
   }
-  g_num_sms = sms > 0 ? sms : 148;
+  g_num_sms = sms > 0 ? sms : 132;
   g_dev_state = 1;
   return MIMO_OK;
 }
 int num_sms() { return g_num_sms; }
 
-static bool g_pdl = false;  // measured on one B200 (power-capped): 1775 ms per clip off, 1800 ms on (profiles/r02_pdl_ab.txt)
+static bool g_pdl = false;  // off unless mimo_debug_pdl(1) / MIMO_B200_PDL=1
 bool pdl_enabled() { return g_pdl; }
 
 static PFN_cuTensorMapEncodeTiled_v12000 g_encode = nullptr;
@@ -93,7 +93,7 @@ int encode_tmap(CUtensorMap* out, int dtype, int rank, const void* base, const u
 
 }  // namespace mimo
 
-extern "C" const char* mimo_version(void) { return "mimo_b200 0.1.0 (sm_100a)"; }
+extern "C" const char* mimo_version(void) { return "mimo_b200 0.1.0 (sm_90a)"; }
 extern "C" const char* mimo_last_error(void) { return mimo::g_err; }
 
 extern "C" int mimo_abi_sizeof(int which) {
@@ -117,9 +117,10 @@ extern "C" int mimo_device_check(int dev) {
     return MIMO_ERR_DEVICE;
   }
   if (dev < 0 || dev >= count) return mimo::set_error(MIMO_ERR_ARG, "mimo_device_check: bad device index");
-  int major = 0;
+  int major = 0, minor = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-  if (major != 10) return mimo::set_error(MIMO_ERR_DEVICE, "device is not sm_100 (B200)");
+  cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
+  if (major != 9 || minor != 0) return mimo::set_error(MIMO_ERR_DEVICE, "device is not sm_90 (H100)");
   return MIMO_OK;
 }
 

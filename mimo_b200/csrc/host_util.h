@@ -10,7 +10,7 @@ namespace mimo {
 
 int set_error(int code, const char* msg);
 int set_cuda_error(const char* what, cudaError_t e);
-// MIMO_OK if the current device is sm_100 (cached per process); error otherwise.
+// MIMO_OK if the current device is sm_90 (cached per process); error otherwise.
 int ensure_device();
 int num_sms();
 // rank-`rank` tiled tensor map, 16-bit elements, 128-byte swizzle, zero OOB fill.
@@ -22,11 +22,10 @@ inline unsigned div_up(long long a, long long b) { return static_cast<unsigned>(
 
 // Programmatic dependent launch (mimo_debug_pdl / MIMO_B200_PDL=1; default OFF): every kernel of the library can be
 // launched with programmatic stream serialization; it begins with griddepcontrol.launch_dependents and, after its
-// shared-memory / TMEM prologue, griddepcontrol.wait, so the next kernel's launch latency and prologue overlap the tail
+// shared-memory prologue, griddepcontrol.wait, so the next kernel's launch latency and prologue overlap the tail
 // of the previous one (~14 000 kernel boundaries per clip). Correctness does not depend on it: the wait is a full
 // dependency on the previous grid (completion + memory visibility); without the attribute both instructions are no-ops.
-// Measured on one power-capped B200 it did not pay: 1800 ms per clip with it, 1775 ms without (the SM clock under the
-// 1 kW cap drops by the same 1.3 % the removed gaps would have gained) - kept as a switch for launch-bound regimes.
+// Off by default; kept as a switch for launch-bound regimes.
 bool pdl_enabled();
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {

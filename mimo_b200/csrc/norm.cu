@@ -15,8 +15,8 @@ namespace mimo {
 //           memory -> one thread per group) and publishes them: part[image][slab][group][2]
 //   pass 2: every block sums the slabs' partials of its image in the same fixed order (bit-identical statistics in
 //           every block and run to run), then normalises + affine (+ SiLU) with 128-bit loads / stores.
-// (A one-pass variant that kept the slab in registers across a per-image arrival barrier was measured at 1.5 TB/s on
-// the 64x64 level - the barrier serialises the blocks of an image - against 2.2 TB/s for these two full-width passes.)
+// (A one-pass variant that keeps the slab in registers across a per-image arrival barrier serialises the blocks of an
+// image on that barrier, and deadlocks when an image has more slabs than blocks can be resident.)
 // ------------------------------------------------------------------------------------------------
 struct GnArgs {
   const void* x0;

@@ -1,5 +1,6 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA, TMEM
-// alloc/ld/st, commit, fences). No CUTLASS/CuTe dependency: these are the only "library" this engine has.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma fences / groups / descriptors
+// (the instructions themselves are in wgmma.cuh). No CUTLASS/CuTe dependency: these are the only "library" this
+// engine has.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_bf16.h>
@@ -68,17 +69,15 @@ __device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
 }
 // Bounded spin: a protocol bug must surface as a trapped kernel (cudaErrorLaunchFailure), never as a
 // hung GPU. try_wait suspends for a HW-defined interval per probe, so the bound is seconds, not ms.
+// (No printf here: a function call inside a wgmma loop makes ptxas serialize every wgmma of the kernel.)
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 26)) {
-      printf("mimo: mbarrier wait timeout (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-      __trap();
-    }
+    if (++spins > (1u << 26)) __trap();
   }
 }
 
-// generic-proxy writes (st.shared) -> visible to the async proxy (TMA store / tcgen05.mma operand reads)
+// generic-proxy writes (st.shared) -> visible to the async proxy (TMA store / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -135,52 +134,29 @@ __device__ __forceinline__ void tma_store_wait_read0() { asm volatile("cp.async.
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------------
-// tcgen05: TMEM management
+// wgmma (warpgroup MMA): fences, groups, shared-memory matrix descriptors, register reallocation
 // ------------------------------------------------------------------------------------------------
-// Whole-warp, .sync.aligned. ncols: power of two in [32, 512]. Base address is written to *smem_dst.
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// Before the first wgmma of a batch: orders earlier register / shared-memory accesses of the warpgroup before it.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// at most N committed groups of this warp still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// tcgen05.commit: arrive(1) on the mbarrier once all previously issued MMAs of this thread retire.
-// Implies tcgen05.fence::before_thread_sync.
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
+// Accumulator registers pass through an empty asm so the compiler does not move their reads or writes across a
+// wgmma_wait (the instructions above take them as "+f" operands, which it cannot see into).
+template <int N>
+__device__ __forceinline__ void reg_fence(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ------------------------------------------------------------------------------------------------
-// tcgen05.mma descriptors
-// ------------------------------------------------------------------------------------------------
-// Instruction descriptor, kind::f16, fp32 accumulate (layout: cute/arch/mma_sm100_desc.hpp:412-434
-// in the vendored CUTLASS headers; restated, not included).
-//   [4,6) c_format (1 = F32)   [7,10) a_format  [10,13) b_format (0 = F16, 1 = BF16)
-//   [15] a_major [16] b_major (0 = K-major, 1 = MN-major)   [17,23) N>>3   [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N, bool bf16, bool a_mn_major,
-                                                      bool b_mn_major) {
-  return (1u << 4) | ((bf16 ? 1u : 0u) << 7) | ((bf16 ? 1u : 0u) << 10) |
-         ((a_mn_major ? 1u : 0u) << 15) | ((b_mn_major ? 1u : 0u) << 16) |
-         (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-}
-// Shared-memory matrix descriptor, 128-byte swizzle (tile rows are 128 B = 64 x 16-bit, 8-row / 1024-B
-// swizzle atoms; the tile base must be 1024-B aligned):
+// Shared-memory matrix descriptor, 128-byte swizzle (tile rows are 128 B = 64 x 16-bit, 8-row / 1024-B swizzle atoms;
+// the tile base must be 1024-B aligned):
 //   [0,14) start address >> 4   [16,30) leading byte offset >> 4   [32,46) stride byte offset >> 4
-//   [46,48) version = 1 (Blackwell)   [61,64) layout type = 2 (SWIZZLE_128B)
-// K-major operand:  LBO unused (1), SBO = 1024 B (next 8-row group).
+//   [62,64) layout type = 1 (SWIZZLE_128B)
+// K-major operand:  LBO unused (1), SBO = 1024 B (next 8-row group); +32 B along K inside the row advances 16 elements.
 // MN-major operand: LBO = byte distance between 64-element chunks along MN, SBO = 1024 B (next 8 K rows).
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
                                                          uint32_t sbo_bytes) {
@@ -188,83 +164,8 @@ __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uin
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
-}
-
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                        uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b,
-                                        uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// ------------------------------------------------------------------------------------------------
-// TMEM <-> registers. Warp w of the CTA may only touch TMEM lanes [32*(w%4), 32*(w%4)+32).
-// 32x32b: thread t of the warp owns lane 32*(w%4)+t; .xN = N consecutive 32-bit columns.
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-        "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st_x32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]),
-      "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]),
-      "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]),
-      "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]),
-      "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_x16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]),
-      "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]),
-      "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -1,4 +1,4 @@
-"""The B200 denoising engine: packs a reference-layout state dict once, then runs the reference's module graph
+"""The H100 denoising engine: packs a reference-layout state dict once, then runs the reference's module graph
 (src/models/unet_3d_edit_bkfill.py:398-576 and friends) as a straight line of C-ABI kernel calls over
 channels-last fp16/bf16 activations. No torch math on the hot path: torch only owns memory and the stream.
 

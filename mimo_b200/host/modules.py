@@ -6,7 +6,7 @@ state-dict keys, forward signatures and error behaviour as
   src/models/pose_guider.py          PoseGuider             (:12-57)
   src/models/mutual_self_attention.py ReferenceAttentionControl (:19-50, :313, :352)
 
-but the modules are only parameter containers: forward() hands the tensors to the sm_100a engine
+but the modules are only parameter containers: forward() hands the tensors to the sm_90a engine
 (mimo_b200/engine.py) through the C ABI. On a non-CUDA device forward() raises — there is no CPU path.
 """
 from __future__ import annotations
@@ -95,7 +95,7 @@ class _EngineModel(nn.Module):
 
     def _require_cuda(self):
         if self.device.type != "cuda":
-            raise MimoError(f"{type(self).__name__}.forward needs the model on a CUDA (sm_100a) device; it is on "
+            raise MimoError(f"{type(self).__name__}.forward needs the model on a CUDA (sm_90a) device; it is on "
                             f"{self.device}. mimo_b200 has no CPU fallback.")
         if self.dtype not in (torch.float16, torch.bfloat16):
             raise MimoError(f"{type(self).__name__}: engine dtypes are float16 / bfloat16, got {self.dtype}")

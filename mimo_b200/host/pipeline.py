@@ -1,5 +1,5 @@
 """Pose2VideoPipeline with the reference's call surface (src/pipelines/pipeline_pose2vid_long_edit_bkfill_roiclip.py:
-36-80 constructor, :338-363 __call__ signature, :573-578 output), driving the sm_100a engine.
+36-80 constructor, :338-363 __call__ signature, :573-578 output), driving the sm_90a engine.
 
 What stays as in the reference: PIL pre-processing semantics, CLIP through the HF module the caller passes, the CPU
 generator noise (prepare_latents :149-183), context windows (:492-510), CFG (:545-549) and DDIM (:551-553) maths.
@@ -248,7 +248,7 @@ class Pose2VideoPipeline:
         key = (p.device, p.dtype, p.data_ptr())
         if getattr(self, "_clip_engine_key", None) != key:
             if p.device.type != "cuda":
-                raise MimoError("the CLIP image encoder must be on a CUDA (sm_100a) device: no CPU fallback")
+                raise MimoError("the CLIP image encoder must be on a CUDA (sm_90a) device: no CPU fallback")
             self._clip_engine = CLIPVisionEngine(self.image_encoder.state_dict(), self.image_encoder.config, p.device, p.dtype)
             self._clip_engine_key = key
         return self._clip_engine
@@ -532,7 +532,7 @@ class Pose2VideoPipeline:
                  context_overlap=4, context_batch_size=1, interpolation_factor=1, **kwargs):
         device = self.device
         if device.type != "cuda":
-            raise MimoError("Pose2VideoPipeline needs its models on a CUDA (sm_100a) device: no CPU fallback")
+            raise MimoError("Pose2VideoPipeline needs its models on a CUDA (sm_90a) device: no CPU fallback")
         if eta != 0.0 or context_batch_size != 1 or interpolation_factor not in (0, 1) or num_images_per_prompt != 1:
             raise NotImplementedError("eta != 0, context_batch_size != 1, interpolation_factor >= 2 and "
                                       "num_images_per_prompt != 1 are outside the reference's shipped configuration")

@@ -10,7 +10,7 @@ One process per GPU. A clip offers three communication-free axes and one that ne
 
 ShardPlan picks (cfg_ways, win_ways, frame_ways) with cfg_ways * win_ways * frame_ways == world: whole windows
 first, then frames, the CFG pair last (it is free of communication but unbalanced: the conditional branch attends to
-twice the keys; measured on 2 GPUs it cost 16 % idle time against ~5 % for the frame exchange).
+twice the keys, so the unconditional GPU waits for the conditional one at every step).
 torch.distributed is used for bootstrap only (exchanging 64-byte IPC handles) and for the once-per-clip gathers.
 """
 from __future__ import annotations
@@ -37,7 +37,7 @@ class ShardPlan:
              min_tokens: Optional[int] = None) -> "ShardPlan":
         """Windows first (communication-free, balanced), then frames (one exchange pair per motion module, balanced),
         the CFG pair last: it needs no exchange but is UNBALANCED - the conditional branch attends to twice the keys at
-        every spatial attention (measured on 2 GPUs: the unconditional GPU idles 16 % of every step), so it is only used
+        every spatial attention (the unconditional GPU waits for the conditional one), so it is only used
         for what the other two axes cannot divide. min_tokens: tokens per frame at the coarsest UNet level (each frame
         group member owns min_tokens / frame_ways of them)."""
         if world < 1 or not 0 <= rank < world:

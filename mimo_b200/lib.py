@@ -1,7 +1,7 @@
 """ctypes binding of libmimo_b200.so (the C ABI declared in include/mimo_b200.h).
 
 Loading never needs a GPU (symbol checks run on CPU); every compute entry point fails loudly without an
-sm_100 device — there is no CPU fallback anywhere in this package.
+sm_90 (H100) device — there is no CPU fallback anywhere in this package.
 """
 from __future__ import annotations
 
@@ -145,9 +145,8 @@ SYMBOLS = {
     "mimo_cfg_ddim_step": (C.c_int, [_VP, _VP, _VP, _I64, _VP, _I64, _F, _F, _F, _F, _F, _I32, _VP]),
 }
 # test hook, not part of the public header
-_DEBUG_SYMBOLS = {"mimo_debug_pdl": (C.c_int, [C.c_int]), "mimo_debug_splitk": (C.c_int, [C.c_int]), "mimo_debug_force_bn": (C.c_int, [C.c_int]), "mimo_debug_attn_variant": (C.c_int, [C.c_int]),
-                  "mimo_debug_attn_trace": (C.c_int, [C.c_void_p]),
-                  "mimo_debug_gemm_trace": (C.c_int, [C.c_void_p])}
+_DEBUG_SYMBOLS = {"mimo_debug_pdl": (C.c_int, [C.c_int]), "mimo_debug_splitk": (C.c_int, [C.c_int]),
+                  "mimo_debug_force_bn": (C.c_int, [C.c_int])}
 
 _lib = None
 

@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE (never imported by mimo_b200/): numpy restatement of run_edit.py's per-frame scene compositing
-(/root/reference/run_edit.py:282-300) — the blend chain after the generated frame has been resized, un-padded and pasted
+(the original project's run_edit.py:282-300) — the blend chain after the generated frame has been resized, un-padded and pasted
 on the white canvas. The loop lives inside MIMO.run, behind TensorFlow / model loading at import time, so it cannot be
 imported; it is restated line by line, with numpy's own type promotion doing the arithmetic, and PINNED against the
 reference's own statements: tests/test_dropin_cpu.py extracts the loop from run_edit.py by AST, executes it with

@@ -2,14 +2,16 @@
 is): a sweep of (step, num_frames, context_size, context_stride, context_overlap, closed_loop) with, per case, the number
 of windows and a CRC-32 of their JSON text (keeps the fixture small), the full lists of a few cases, bit-reversal
 fractions of `ordered_halving`, and `get_total_steps` values.   python oracle/gen_context_golden.py
-Test infrastructure: runs only in the build container (needs /root/reference)."""
+Test infrastructure: needs a checkout of the original project, named by MIMO_REFERENCE."""
 import importlib.util
 import json
+import os
+import sys
 import zlib
 from pathlib import Path
 
 ROOT = Path(__file__).resolve().parents[1]
-REF = Path("/root/reference/src/pipelines/context.py")
+REF = Path(os.environ.get("MIMO_REFERENCE") or sys.exit(__doc__)) / "src" / "pipelines" / "context.py"
 
 
 def sweep_cases():
@@ -41,7 +43,7 @@ def main():
     totals = [[n, frames, size, stride, overlap,
                ref.get_total_steps(sched, list(range(n)), 20, frames, size, stride, overlap)]
               for n in (1, 2, 20, 25) for frames, size, stride, overlap in ((24, 24, 1, 4), (48, 24, 1, 4), (150, 24, 3, 4), (64, 16, 2, 4))]
-    out = {"generator": "oracle/gen_context_golden.py over /root/reference/src/pipelines/context.py",
+    out = {"generator": "oracle/gen_context_golden.py over the original project's src/pipelines/context.py",
            "case_fields": ["step", "num_frames", "context_size", "context_stride", "context_overlap", "closed_loop",
                            "n_windows", "crc32_of_json"],
            "cases": cases, "full": full, "ordered_halving": halving,

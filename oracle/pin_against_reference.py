@@ -1,6 +1,6 @@
 """Pin the functional oracle (oracle/torch_oracle.py) against the reference's OWN code, and write golden fixtures.
 
-Runs only in the build container (needs /root/reference, read-only). It imports /root/reference/src/** verbatim
+Needs a checkout of the original project, named by MIMO_REFERENCE (read-only). It imports its src/** verbatim
 on top of oracle/diffusers_shim, loads the same seeded state dicts into the reference's modules (strict=True: this
 also pins the state-dict key schema) and checks, in fp32 on CPU:
 
@@ -10,12 +10,13 @@ also pins the state-dict key schema) and checks, in fp32 on CPU:
      multi-window case F=26 > 24 frames at low resolution)                                          == oracle
   4. context windows and DDIM timestep tables                                                       == oracle (bit-exact)
 
-then stores inputs-by-seed + expected outputs under tests/golden/ for the GPU parity tests (the GPU box has no
-/root/reference). Usage:  python oracle/pin_against_reference.py [--write]
+then stores inputs-by-seed + expected outputs under tests/golden/ for the GPU parity tests (which run without the
+original project). Usage:  MIMO_REFERENCE=<checkout> python oracle/pin_against_reference.py [--write]
 """
 from __future__ import annotations
 
 import argparse
+import os
 import json
 import sys
 from pathlib import Path
@@ -24,7 +25,7 @@ import numpy as np
 import torch
 
 ROOT = Path(__file__).resolve().parents[1]
-REF = Path("/root/reference")
+REF = Path(os.environ.get("MIMO_REFERENCE") or sys.exit(__doc__))
 sys.path.insert(0, str(ROOT))
 sys.path.insert(0, str(ROOT / "oracle" / "diffusers_shim"))
 sys.path.insert(0, str(REF))

@@ -6,13 +6,13 @@ nothing under mimo_b200/ does. It runs on whatever device its tensors live on (C
 checker may also run it on the GPU in fp32 — it is still torch library code, never our kernels).
 
 Pinning: the reference has no tests, fixtures or golden vectors for this path (SURVEY.md §4/§8c), so this file
-is pinned against *outputs of the reference itself*: oracle/pin_against_reference.py imports /root/reference/src
+is pinned against *outputs of the reference itself*: oracle/pin_against_reference.py imports the original project's src
 verbatim (on oracle/diffusers_shim) in the build container, feeds both implementations the same seeded state
 dicts and inputs, asserts agreement, and writes tests/golden/*.pt. diffusers==0.24.0 (install.sh:12) is absent
-from /root/reference and this image; its Attention / FeedForward / ResnetBlock2D / AutoencoderKL / DDIMScheduler
+from the original project and this image; its Attention / FeedForward / ResnetBlock2D / AutoencoderKL / DDIMScheduler
 arithmetic is restated here from the published algorithm and anchored on the reference's call sites.
 
-Every function cites the reference file:line it follows (paths relative to /root/reference).
+Every function cites the reference file:line it follows (paths relative to the original project's root).
 """
 from __future__ import annotations
 

@@ -113,9 +113,9 @@ def main():
         if rank == 0:
             print(json.dumps(row), flush=True)
         # The way back from pixels to frames rounds proj_out's result to fp16 before the residual add (the un-sharded GEMM
-        # epilogue adds in fp32): 42 extra roundings per forward out of ~700, measured 1.1e-3 on the latents after two
-        # steps; classifier-free guidance (x3.5 on the branch difference) amplifies that to ~3.6e-3. Both are below the
-        # distance between two fp16 executions of the same clip (engine vs PyTorch fp16: 2.3e-3 per forward).
+        # epilogue adds in fp32): 42 extra roundings per forward out of ~700. Classifier-free guidance (x3.5 on the branch
+        # difference) amplifies that difference, hence the looser limit with guidance; both limits sit at the scale of the
+        # distance between two fp16 executions of the same clip (engine vs PyTorch fp16, tests/test_parity_gpu.py).
         lim = 5e-3 if guidance > 1.0 else 2e-3
         ok &= same and same_sh and row["latents_rel_l2"] <= lim and row["videos_rel_l2"] <= 2e-3
     # every rank must hold the same clip

@@ -1,6 +1,6 @@
 """Launch each hot kernel a few times at hot-path shapes so that `ncu -k regex:<name>` can capture it in isolation
 (GPU box only):   ncu --set full --clock-control none --import-source on -k regex:attn_spatial -s 2 -c 1 \
-                      -o gpurun_out/attn python scripts/ncu_kernels.py attn
+                      -o attn python scripts/ncu_kernels.py attn
 """
 from __future__ import annotations
 

@@ -1,5 +1,5 @@
 """Aggregate an `ncu --csv` launch list (gpu__time_duration.sum, dram bytes) per kernel name:
-   python scripts/ncu_launchlist.py gpurun_out/launches.csv > profiles/rNN_launches_summary.txt"""
+   python scripts/ncu_launchlist.py launches.csv > launches_summary.txt"""
 import csv, sys, collections, re
 
 def main(path):

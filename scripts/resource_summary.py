@@ -1,6 +1,6 @@
 """Static resource usage of every kernel instantiation in the in-tree library (runs without a GPU):
 registers / thread, stack bytes (local-memory frame: spills or indexed locals), static shared memory, from
-`cuobjdump --dump-resource-usage`.   python scripts/resource_summary.py > profiles/r02_resource_usage.txt"""
+`cuobjdump --dump-resource-usage`.   python scripts/resource_summary.py > resource_usage.txt"""
 import re
 import subprocess
 import sys
@@ -23,7 +23,7 @@ def main():
         if m and name:
             rows.append((name, *map(int, m.groups())))
             name = None
-    print(f"Resource usage of {LIB.name}: {len(rows)} kernel instantiations (sm_100a)\n"
+    print(f"Resource usage of {LIB.name}: {len(rows)} kernel instantiations (sm_90a)\n"
           "dynamic shared memory is set at launch and not listed; STACK > 0 marks a local-memory frame\n")
     print(f"{'kernel':72s} {'regs':>5s} {'stack':>6s} {'smem':>6s} {'local':>6s}")
     for r in sorted(rows):

@@ -9,7 +9,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (sm_100a) GPU; run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a) GPU; select with -m gpu")
 
 
 @pytest.fixture(scope="session")

@@ -97,3 +97,13 @@ def test_usable_cores_and_extrapolation(bench_mod):
     assert 1 <= b.usable_cores() <= 4096
     fx = {"t_ref": 1.0, "t_dec": 2.0, "t_enc": 3.0}
     assert b._extrapolate(10.0, 8, fx) == 20 * 10.0 * 3 + 24 * 2.0 + 2 * 3.0 + 1.0
+
+
+@pytest.mark.parametrize("argv", [["--steps", "0"], ["--impl", "reference", "--dump-outputs", "d"],
+                                  ["--one-clip", "--dump-outputs", "d"]])
+def test_rejected_argument_combinations(bench_mod, monkeypatch, argv):
+    """--steps must time at least one step, and --dump-outputs only exists for the engine's timed steps."""
+    monkeypatch.setattr("sys.argv", ["bench.py", *argv])
+    with pytest.raises(SystemExit) as e:
+        bench_mod.main()
+    assert e.value.code == 2

@@ -1,5 +1,5 @@
 """CPU-side checks of the drop-in boundary: the library loads without a GPU, exports every symbol the header
-declares, and every compute entry point refuses to run without an sm_100 device (no CPU fallback)."""
+declares, and every compute entry point refuses to run without an sm_90 device (no CPU fallback)."""
 import ctypes
 import re
 from pathlib import Path
@@ -32,7 +32,7 @@ def test_header_symbols_are_exported_and_bound():
 
 def test_version_and_struct_layout():
     lib = L.load()
-    assert b"sm_100a" in lib.mimo_version()
+    assert b"sm_90a" in lib.mimo_version()
     # the ctypes mirrors must match the C structs (pointer + int64 + float layout, natural alignment)
     for which, st in enumerate((L.Epilogue, L.GemmParams, L.Conv3x3Params, L.GroupNormParams, L.AttnParams)):
         assert lib.mimo_abi_sizeof(which) == ctypes.sizeof(st), st.__name__

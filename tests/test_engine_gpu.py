@@ -1,4 +1,4 @@
-"""Engine parity on a B200: whole networks through the C ABI against the oracle (fp32 torch, same fp16-rounded
+"""Engine parity on an H100: whole networks through the C ABI against the oracle (fp32 torch, same fp16-rounded
 weights) and against the golden vectors the reference produced (tests/golden, oracle/pin_against_reference.py).
 
 Stated tolerance (fp16 storage, fp32 accumulate): rel-L2 of a whole UNet forward <= 3e-3 against the fp32 oracle,

@@ -238,7 +238,7 @@ def test_conv_up2x_weight_packing_equals_interpolate_plus_conv():
         for b in range(2):
             for iy in range(2):
                 for ix in range(2):
-                    dy, dx = a - 1 + iy, b - 1 + ix  # the offsets csrc/gemm_tcgen05.cu: mimo_conv_up2x uses
+                    dy, dx = a - 1 + iy, b - 1 + ix  # the offsets csrc/gemm_wgmma.cu: mimo_conv_up2x uses
                     src = xp[:, :, 1 + dy:1 + dy + h, 1 + dx:1 + dx + w]
                     out[:, :, a::2, b::2] += torch.einsum("oc,nchw->nohw", w4[2 * a + b, :, 2 * iy + ix], src)
     assert float((out - ref).abs().max()) < 1e-4

@@ -1,4 +1,4 @@
-"""Per-kernel parity on a B200: every C-ABI kernel against a plain PyTorch fp32 reference of the same op, at the
+"""Per-kernel parity on an H100: every C-ABI kernel against a plain PyTorch fp32 reference of the same op, at the
 exact shapes of the hot path (SURVEY.md §2.2/§9) and at ragged / tail / empty-ish edge shapes.
 Tolerance: rel-L2 <= 2e-3 on fp16 outputs (fp16 rounding of the result is 2^-11 ~ 4.9e-4 relative); integer-valued
 GEMM inputs must come out bit-exact."""

@@ -9,7 +9,80 @@ import numpy as np
 import pytest
 import torch
 
-from test_dropin_cpu import REF, _oracle_engines  # noqa: F401  (same stand-ins as the drop-in proof)
+
+def _oracle_engines(monkeypatch, O, cfg, vcfg):
+    """Stand-ins for the four engine factories, backed by the oracle (fp32, CPU)."""
+    from mimo_b200 import ops
+    from mimo_b200.host import modules as M
+
+    def ncfhw_to_nhwc(src, cpad, dtype, out=None):
+        b, c, f, h, w = src.shape
+        t = src.permute(0, 2, 3, 4, 1).reshape(b * f * h * w, c).to(dtype)
+        return torch.nn.functional.pad(t, (0, cpad - c))
+
+    def nhwc_to_ncfhw(src, b, c, f, h, w, out_dtype=None, out=None):
+        return src[:, :c].reshape(b, f, h, w, c).permute(0, 4, 1, 2, 3).contiguous()
+
+    monkeypatch.setattr(ops, "ncfhw_to_nhwc", ncfhw_to_nhwc)
+    monkeypatch.setattr(ops, "nhwc_to_ncfhw", nhwc_to_ncfhw)
+    monkeypatch.setattr(M._EngineModel, "_require_cuda", lambda self: None)
+
+    class Den:
+        def __init__(self, sd):
+            self.sd, self.clip_state = sd, None
+
+        def begin_clip(self, ehs, banks, cfg, frames, branches=None):
+            self.clip_state = {"ehs": ehs, "banks": banks, "cfg": cfg}
+
+        def set_cross_attn(self, ehs):
+            self.clip_state["ehs"] = ehs
+
+        def forward(self, sample, timestep, pose_nhwc):
+            b, c, f, h, w = sample.shape
+            pose = pose_nhwc.reshape(b, f, h, w, -1).permute(0, 4, 1, 2, 3)
+            st = self.clip_state
+            # the host layer hands over the conditional half of the banks only (the unconditional half is never read);
+            # the oracle restates the reference, which keeps both: fill the unused slot with a copy
+            banks = {k: (v if v.shape[0] == b else v.repeat(b, 1, 1)) for k, v in st["banks"].items()}
+            return O.denoising_unet(self.sd, sample, int(timestep), st["ehs"], pose, banks, cfg, cfg=st["cfg"])
+
+    class Ref:
+        def __init__(self, sd):
+            self.sd = sd
+
+        def write_banks(self, latents, ehs, reader):
+            return O.reference_unet_banks(self.sd, latents, ehs, cfg)
+
+    class Pose:
+        def __init__(self, sd):
+            self.sd = sd
+
+        def forward(self, cond):
+            y = O.pose_guider(self.sd, cond)  # [b, C, F, h, w]
+            return y.permute(0, 2, 3, 4, 1).reshape(-1, y.shape[1])
+
+    class Vae:
+        def __init__(self, sd):
+            self.sd = sd
+
+        def encode_mean(self, x):
+            return O.vae_encode_mean(self.sd, x, vcfg)
+
+        def decode(self, z):
+            return O.vae_decode(self.sd, z, vcfg)
+
+    def cached(factory):
+        def engine(self):
+            if self._engine is None:
+                self._engine = factory(self.state_dict())
+            return self._engine
+        return engine
+
+    monkeypatch.setattr(M.UNet3DConditionModel, "engine", cached(Den))
+    monkeypatch.setattr(M.UNet2DConditionModel, "engine", cached(Ref))
+    monkeypatch.setattr(M.PoseGuider, "engine", cached(Pose))
+    monkeypatch.setattr(M.AutoencoderKL, "engine", cached(lambda sd: (Vae(sd), Vae(sd))))
+
 
 
 class _Event:
