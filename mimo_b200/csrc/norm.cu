@@ -11,10 +11,13 @@ namespace mimo {
 
 // ------------------------------------------------------------------------------------------------
 // GroupNorm(+SiLU), deterministic: two streaming kernels, no floating-point atomics.
-//   pass 1: every block reduces its slab of pixels to per-group (sum, sumsq) in a FIXED order (registers -> shared
-//           memory -> one thread per group) and publishes them: part[image][slab][group][2]
+//   pass 1: every block reduces its slab of pixels to per-group (sum, sumsq) of x - K_g in a FIXED order (registers ->
+//           shared memory -> one thread per group) and publishes them: part[image][slab][group][2]
 //   pass 2: every block sums the slabs' partials of its image in the same fixed order (bit-identical statistics in
 //           every block and run to run), then normalises + affine (+ SiLU) with 128-bit loads / stores.
+// K_g is one sample of the group (gn_shift). Without it, var = E[x^2] - mean^2 cancels nearly all of fp32's digits once
+// |mean| >> std (at mean / std = 300 the output was off by ~1.5 % rel-L2); with it both terms are of the order of the
+// variance, as in a two-pass computation, at the cost of a few cached scalar loads per block.
 // (A one-pass variant that keeps the slab in registers across a per-image arrival barrier serialises the blocks of an
 // image on that barrier, and deadlocks when an image has more slabs than blocks can be resident.)
 // ------------------------------------------------------------------------------------------------
@@ -24,7 +27,7 @@ struct GnArgs {
   const void* gamma;
   const void* beta;
   void* out;
-  float* part;  // [n][bpi][groups][2] = (sum, sumsq) per slab
+  float* part;  // [n][bpi][groups][2] = (sum, sumsq) of x - K_g per slab
   int c0, c1, C, hw, groups, cpg;
   int vecs;  // C / 8
   int P;     // pixels processed side by side by one block
@@ -42,6 +45,18 @@ __device__ __forceinline__ uint4 gn_load(const GnArgs& a, long long pix, int cv)
     return *reinterpret_cast<const uint4*>(static_cast<const typename C::T*>(a.x0) + pix * a.c0 + ch);
   }
   return *reinterpret_cast<const uint4*>(static_cast<const typename C::T*>(a.x1) + pix * a.c1 + (ch - a.c0));
+}
+
+// K_g: image n's first pixel in group g's first channel. Both passes read the same element, so every block shifts by
+// the same value.
+template <bool kBf16>
+__device__ __forceinline__ float gn_shift(const GnArgs& a, int n, int g) {
+  using C = Cvt<kBf16>;
+  const int ch = g * a.cpg;
+  const long long pix = static_cast<long long>(n) * a.hw;
+  const typename C::T* p = ch < a.c0 ? static_cast<const typename C::T*>(a.x0) + pix * a.c0 + ch
+                                     : static_cast<const typename C::T*>(a.x1) + pix * a.c1 + (ch - a.c0);
+  return C::to_f(*p);
 }
 
 constexpr int kGnMaxThreads = 320;
@@ -64,6 +79,7 @@ __global__ void __launch_bounds__(kGnMaxThreads) gn_stats_kernel(GnArgs a) {
   if (split > 8) split = 8;
   float sA = 0.f, qA = 0.f, sB = 0.f, qB = 0.f;
   if (active) {
+    const float kA = gn_shift<kBf16>(a, n, gA), kB = split < 8 ? gn_shift<kBf16>(a, n, gA + 1) : 0.f;
     const int p_begin = blockIdx.x * a.pix_per_block;
     int p_end = p_begin + a.pix_per_block;
     if (p_end > a.hw) p_end = a.hw;
@@ -74,8 +90,20 @@ __global__ void __launch_bounds__(kGnMaxThreads) gn_stats_kernel(GnArgs a) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const float2 t = C::unpack(w[j]);
-        if (2 * j < split) sA += t.x, qA += t.x * t.x; else sB += t.x, qB += t.x * t.x;
-        if (2 * j + 1 < split) sA += t.y, qA += t.y * t.y; else sB += t.y, qB += t.y * t.y;
+        if (2 * j < split) {
+          const float d = t.x - kA;
+          sA += d, qA += d * d;
+        } else {
+          const float d = t.x - kB;
+          sB += d, qB += d * d;
+        }
+        if (2 * j + 1 < split) {
+          const float d = t.y - kA;
+          sA += d, qA += d * d;
+        } else {
+          const float d = t.y - kB;
+          sB += d, qB += d * d;
+        }
       }
     }
   }
@@ -111,6 +139,8 @@ __global__ void __launch_bounds__(kGnMaxThreads) gn_apply_kernel(GnArgs a) {
   const int tid = threadIdx.x;
   const int g2 = a.groups * 2;
   {
+    // K_g first (the same thread adds the shifted mean below): the load overlaps the partial sums
+    for (int g = tid; g < a.groups; g += blockDim.x) s_mean[g] = gn_shift<kBf16>(a, n, g);
     const int parts = a.bpi >= 16 ? 4 : 1;  // a function of the shape only: the summation order never varies
     const float* src = a.part + static_cast<long long>(n) * a.bpi * g2;
     for (int idx = tid; idx < parts * g2; idx += blockDim.x) {
@@ -127,10 +157,10 @@ __global__ void __launch_bounds__(kGnMaxThreads) gn_apply_kernel(GnArgs a) {
         s += s_tot[part][2 * g];
         q += s_tot[part][2 * g + 1];
       }
-      const float mean = s * inv_cnt;
-      float var = q * inv_cnt - mean * mean;
+      const float dmean = s * inv_cnt;  // mean of x - K_g
+      float var = q * inv_cnt - dmean * dmean;
       var = var < 0.f ? 0.f : var;
-      s_mean[g] = mean;
+      s_mean[g] += dmean;
       s_rstd[g] = rsqrtf(var + a.eps);
     }
     __syncthreads();
@@ -142,24 +172,28 @@ __global__ void __launch_bounds__(kGnMaxThreads) gn_apply_kernel(GnArgs a) {
   const int gA = ch0 / a.cpg;
   int split = (gA + 1) * a.cpg - ch0;
   if (split > 8) split = 8;
-  float sc[8], sh[8];
+  // y = (x - mean) * (rstd * gamma) + beta. The folded form x * sc + (beta - mean * sc) cancels: both terms are of the
+  // order |mean| * rstd, which reaches 1e6 for a near-constant group at mean 1000 (eps 1e-6), so its fp32 rounding
+  // alone moved the output by 0.06. x - mean is exact or nearly so.
+  float sc[8], bc[8], mA, mB;
   {
     const uint4 ug = *reinterpret_cast<const uint4*>(static_cast<const typename C::T*>(a.gamma) + ch0);
     const uint4 ub = *reinterpret_cast<const uint4*>(static_cast<const typename C::T*>(a.beta) + ch0);
     const uint32_t wg[4] = {ug.x, ug.y, ug.z, ug.w};
     const uint32_t wb[4] = {ub.x, ub.y, ub.z, ub.w};
-    const float mA = s_mean[gA], rA = s_rstd[gA];
-    const float mB = split < 8 ? s_mean[gA + 1] : 0.f, rB = split < 8 ? s_rstd[gA + 1] : 0.f;
+    const float rA = s_rstd[gA], rB = split < 8 ? s_rstd[gA + 1] : 0.f;
+    mA = s_mean[gA];
+    mB = split < 8 ? s_mean[gA + 1] : 0.f;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const float2 gg = C::unpack(wg[j]);
       const float2 bb = C::unpack(wb[j]);
-      const float m0 = 2 * j < split ? mA : mB, r0 = 2 * j < split ? rA : rB;
-      const float m1 = 2 * j + 1 < split ? mA : mB, r1 = 2 * j + 1 < split ? rA : rB;
+      const float r0 = 2 * j < split ? rA : rB;
+      const float r1 = 2 * j + 1 < split ? rA : rB;
       sc[2 * j] = r0 * gg.x;
-      sh[2 * j] = bb.x - m0 * r0 * gg.x;
+      bc[2 * j] = bb.x;
       sc[2 * j + 1] = r1 * gg.y;
-      sh[2 * j + 1] = bb.y - m1 * r1 * gg.y;
+      bc[2 * j + 1] = bb.y;
     }
   }
   const int p_begin = blockIdx.x * a.pix_per_block;
@@ -174,8 +208,8 @@ __global__ void __launch_bounds__(kGnMaxThreads) gn_apply_kernel(GnArgs a) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const float2 t = C::unpack(w[j]);
-      f[2 * j] = fmaf(t.x, sc[2 * j], sh[2 * j]);
-      f[2 * j + 1] = fmaf(t.y, sc[2 * j + 1], sh[2 * j + 1]);
+      f[2 * j] = fmaf(t.x - (2 * j < split ? mA : mB), sc[2 * j], bc[2 * j]);
+      f[2 * j + 1] = fmaf(t.y - (2 * j + 1 < split ? mA : mB), sc[2 * j + 1], bc[2 * j + 1]);
     }
     if (a.silu) {
 #pragma unroll

@@ -56,11 +56,18 @@ def gemm_case(M, N, K, bn=0, dtype=torch.float16, **kw):
     torch.manual_seed(M * 7 + N * 3 + K)
     a = ints((M, K), dtype=dtype)
     w = ints((N, K), dtype=dtype)
-    out = ops.gemm(a, w)
-    torch.cuda.synchronize()
-    ref = a.float() @ w.float().t()
+    try:
+        out = ops.gemm(a, w)
+        torch.cuda.synchronize()
+    finally:
+        lib.mimo_debug_force_bn(0)
+    ref = a.double() @ w.double().t()
     ok = report(f"gemm M={M} N={N} K={K} bn={bn}", out, ref, tol=1e-3)
-    lib.mimo_debug_force_bn(0)
+    # integer inputs: every fp32 partial sum is exact, so the output is the exact product rounded once
+    bad = int((out != ref.to(out.dtype)).sum())
+    if bad:
+        print(f"[FAIL] gemm M={M} N={N} K={K} bn={bn}: not bit-exact, {bad}/{out.numel()} elements differ")
+    ok &= bad == 0
     return ok, a, w, out, ref
 
 
