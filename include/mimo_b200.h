@@ -248,6 +248,13 @@ int mimo_nhwc_to_ncfhw(const void* src, void* dst, int32_t b, int32_t c, int32_t
                        int32_t ld, int32_t dst_is_f32, int32_t dtype, void* stream);
 /* nearest-neighbour x2 upsampling of [n, h, w, c] -> [n, 2h, 2w, c] (F.interpolate in Upsample3D, resnet.py:70-73) */
 int mimo_upsample2x(const void* x, void* out, int32_t n, int32_t h, int32_t w, int32_t c, int32_t dtype, void* stream);
+/* nearest-neighbour resize of [n, h, w, c] -> [n, oh, ow, c] to any size, bit-identical to F.interpolate(mode="nearest",
+ * size=(oh, ow)): source row min(floor(oy * (float(h) / oh)), h - 1) in fp32, columns alike. Replaces the forwarded-size
+ * interpolation of Upsample3D / Upsample2D (src/models/resnet.py:75-77) that the UNets run when a latent side is not a
+ * multiple of 8 (src/models/unet_3d_edit_bkfill.py:427-435, 544-545; unet_2d_condition.py:946-955, 1269-1270).
+ * Requirements: c % 8 == 0, 16-byte aligned x and out. */
+int mimo_upsample_nearest(const void* x, void* out, int32_t n, int32_t h, int32_t w, int32_t oh, int32_t ow, int32_t c,
+                          int32_t dtype, void* stream);
 /* in-place row softmax of x[rows, cols] (leading dim ld), fp32 math: the VAE mid-block attention (1 head, d=512) is
  * run as GEMM -> softmax -> GEMM (diffusers AttnProcessor2_0 on UNetMidBlock2D's Attention). */
 int mimo_softmax_rows(void* x, int64_t rows, int32_t cols, int64_t ld, int32_t dtype, void* stream);

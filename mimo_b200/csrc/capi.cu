@@ -93,7 +93,7 @@ int encode_tmap(CUtensorMap* out, int dtype, int rank, const void* base, const u
 
 }  // namespace mimo
 
-extern "C" const char* mimo_version(void) { return "mimo_b200 0.1.0 (sm_90a)"; }
+extern "C" const char* mimo_version(void) { return "mimo_b200 0.2.0 (sm_90a)"; }
 extern "C" const char* mimo_last_error(void) { return mimo::g_err; }
 
 extern "C" int mimo_abi_sizeof(int which) {

@@ -114,6 +114,26 @@ __global__ void upsample2x_kernel(const uint4* __restrict__ x, uint4* __restrict
   }
 }
 
+// nearest resize to any (oh, ow), channels-last: one thread per output (pixel, 8-channel vector). The source index is
+// PyTorch's for F.interpolate(mode="nearest", size=...): floor(d * (float(in) / out)) in fp32, clamped to in - 1.
+__global__ void upsample_nearest_kernel(const uint4* __restrict__ x, uint4* __restrict__ out, int n, int h, int w,
+                                        int oh, int ow, int vecs, float sy, float sx) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const long long total = static_cast<long long>(n) * oh * ow * vecs;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int cv = static_cast<int>(i % vecs);
+    const long long opix = i / vecs;
+    const int ox = static_cast<int>(opix % ow);
+    const int oy = static_cast<int>((opix / ow) % oh);
+    const long long ni = opix / (static_cast<long long>(ow) * oh);
+    const int iy = min(static_cast<int>(floorf(__fmul_rn(static_cast<float>(oy), sy))), h - 1);
+    const int ix = min(static_cast<int>(floorf(__fmul_rn(static_cast<float>(ox), sx))), w - 1);
+    out[i] = x[((ni * h + iy) * w + ix) * vecs + cv];
+  }
+}
+
 // in-place row softmax, one CTA per row, fp32 math
 template <bool kBf16>
 __global__ void __launch_bounds__(256) softmax_rows_kernel(void* __restrict__ xp, int cols, long long ld) {
@@ -320,6 +340,27 @@ extern "C" int mimo_upsample2x(const void* x, void* out, int32_t n, int32_t h, i
   const long long total = static_cast<long long>(n) * 4 * h * w * (c / 8);
   upsample2x_kernel<<<ew_grid(total, 256), 256, 0, st>>>(static_cast<const uint4*>(x), static_cast<uint4*>(out), n, h, w, c / 8);
   MIMO_CHECK_LAUNCH("upsample2x launch");
+  return MIMO_OK;
+}
+
+extern "C" int mimo_upsample_nearest(const void* x, void* out, int32_t n, int32_t h, int32_t w, int32_t oh, int32_t ow,
+                                     int32_t c, int32_t dtype, void* stream) {
+  if (!x || !out) return set_error(MIMO_ERR_ARG, "mimo_upsample_nearest: null pointer");
+  if (n <= 0 || h <= 0 || w <= 0 || oh <= 0 || ow <= 0 || c <= 0 || (c % 8))
+    return set_error(MIMO_ERR_ARG, "mimo_upsample_nearest: sizes must be positive and c a multiple of 8");
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out)) & 15)
+    return set_error(MIMO_ERR_ARG, "mimo_upsample_nearest: x and out must be 16-byte aligned");
+  if (dtype != MIMO_F16 && dtype != MIMO_BF16) return set_error(MIMO_ERR_ARG, "mimo_upsample_nearest: bad dtype");
+  if (int rc = ensure_device()) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long total = static_cast<long long>(n) * oh * ow * (c / 8);
+  // the same fp32 quotient PyTorch's kernel uses (compute_scales_value without a scale factor: in / out)
+  const float sy = static_cast<float>(h) / static_cast<float>(oh);
+  const float sx = static_cast<float>(w) / static_cast<float>(ow);
+  cudaError_t e = launch_k(upsample_nearest_kernel, dim3(ew_grid(total, 256)), dim3(256), 0, st,
+                           static_cast<const uint4*>(x), static_cast<uint4*>(out), n, h, w, oh, ow, c / 8, sy, sx);
+  if (e == cudaSuccess) e = cudaGetLastError();
+  if (e != cudaSuccess) return set_cuda_error("upsample_nearest launch", e);
   return MIMO_OK;
 }
 

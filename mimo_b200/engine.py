@@ -89,6 +89,20 @@ class _Packer:
         return ops.pack_conv_up2x_weight(self.t(p + ".weight")), self.t(p + ".bias")
 
 
+def latent_levels(h: int, w: int, levels: int) -> List[Tuple[int, int]]:
+    """(h, w) of the latent at each of the UNet's `levels` resolutions, finest first. Every Downsample3D / Downsample2D is
+    a 3x3 conv with stride 2 and padding 1 (resnet.py:93-120), so a level is ceil(s / 2) of the one above: 98 -> 49 ->
+    25 -> 13. The up path returns to exactly these sizes (the reference interpolates each upsampler to the size of the
+    skip tensor it meets, unet_3d_edit_bkfill.py:544-545)."""
+    if h <= 0 or w <= 0:
+        raise L.MimoError(f"latent size {h} x {w} is empty")
+    out = [(h, w)]
+    for _ in range(levels - 1):
+        h, w = (h + 1) // 2, (w + 1) // 2
+        out.append((h, w))
+    return out
+
+
 def bank_index_rows(branches: Sequence[int], frames: int, cfg: bool, nbank: int):
     """Bank routing of every frame-sample row of a forward (mutual_self_attention.py:154-197): -1 = attend to self only
     (the unconditional CFG branch), else the index of the bank feature map to append. With CFG the conditional bank is the
@@ -204,7 +218,10 @@ class UNetEngine:
                 if spec.motion:
                     add_mm(f"up_blocks.{i}.motion_modules.{j}")
             if i < nb - 1:
+                # both forms of the upsampler's conv: parity classes for an exact x2 step, the plain [Cout, 9 Cin] packing
+                # behind a general resize (a level whose target is 2s - 1 on some axis, see _up)
                 W[f"up_blocks.{i}.up"] = pk.conv_up(f"up_blocks.{i}.upsamplers.0.conv")
+                W[f"up_blocks.{i}.up_conv"] = pk.conv3(f"up_blocks.{i}.upsamplers.0.conv")
         if spec.out_head:
             W["norm_out"] = pk.norm("conv_norm_out")
             W["conv_out"] = pk.conv3("conv_out")
@@ -321,20 +338,29 @@ class UNetEngine:
         col = ops.im2col3x3(x, n, h, w, stride=2)
         return ops.gemm(col, wp, bias=b)
 
-    def _up(self, p, x, n, h, w):
-        wp, b = self.w[p]
-        return ops.conv_up2x(x, wp, n, h, w, bias=b)  # Upsample3D (resnet.py:53-90) without the 4x tensor
+    def _up(self, p, x, n, h, w, th, tw):
+        """Upsample3D (resnet.py:53-90) from (h, w) to the skip tensor's (th, tw). An exact x2 step runs the fused
+        nearest-x2 + 3x3 kernel without the 4x tensor. Otherwise th or tw is 2s - 1 (ceil halving on the way down): the
+        nearest resize is materialised and convolved with zero padding after its last row / column, which the fused
+        kernel's parity taps cannot express (they would read source row s - 1 there)."""
+        if (th, tw) == (2 * h, 2 * w):
+            wp, b = self.w[p]
+            return ops.conv_up2x(x, wp, n, h, w, bias=b)
+        wp, b = self.w[p + "_conv"]
+        return ops.conv3x3(ops.upsample_nearest(x, n, h, w, th, tw), wp, n, th, tw, bias=b)
 
     def check_latent_size(self, h: int, w: int) -> None:
-        """The down path halves h and w once per level and the up path doubles them back exactly. The reference also
-        accepts sizes that do not divide (its script default 784 x 784 -> 98 x 98 latents) by interpolating every upsampler
-        to the skip connection's size (unet_3d_edit_bkfill.py:430-435, :544-545 `forward_upsample_size`); the fused
-        nearest-x2 + 3x3 kernel (mimo_conv_up2x) has no such mode: refuse instead of reading past the skip tensors."""
+        """Whether the fused nearest-x2 + 3x3 kernel (mimo_conv_up2x) serves every level: the down path then halves h and
+        w exactly and every up step doubles them back. Other sizes (the reference's script default 784 x 784 -> 98 x 98
+        latents) take the reference's `forward_upsample_size` path (unet_3d_edit_bkfill.py:430-435, :544-545) at the levels
+        that do not double exactly; forward() and write_banks() run both."""
         m = 1 << (len(self.spec.block_out_channels) - 1)
         if h <= 0 or w <= 0 or h % m or w % m:
-            raise L.MimoError(f"latent size {h} x {w} is not a multiple of {m} (pixels: {8 * m}): the reference's "
-                              "forward_upsample_size path (unet_3d_edit_bkfill.py:430-435) is not implemented; "
-                              f"use a width and height that are multiples of {8 * m}")
+            raise L.MimoError(f"latent size {h} x {w} is not a multiple of {m} (pixels: {8 * m}): some up steps take the "
+                              "forward_upsample_size path (unet_3d_edit_bkfill.py:430-435) instead of the fused x2 kernel")
+
+    def levels(self, h: int, w: int) -> List[Tuple[int, int]]:
+        return latent_levels(h, w, len(self.spec.block_out_channels))
 
     xchg = None  # host.shard.Exchange of this GPU's frame group (None / G == 1: all frames of a window are local)
     taps: Optional[dict] = None  # debugging aid (scripts/gpu_probe.py): block outputs as [N, C, H, W] fp32 on CPU
@@ -348,6 +374,7 @@ class UNetEngine:
         sp = self.spec
         nb = len(sp.block_out_channels)
         n = b * f
+        lv = latent_levels(h, w, nb)
         skips = [(x, h, w)]
         rpb = lambda hh, ww: f * hh * ww  # rows per CFG branch at this resolution
         for i in range(nb):
@@ -360,7 +387,7 @@ class UNetEngine:
                 skips.append((x, h, w))
             if i < nb - 1:
                 x = self._down(f"down_blocks.{i}.down", x, n, h, w)
-                h, w = h // 2, w // 2
+                h, w = lv[i + 1]
                 self._tap(f"down_blocks.{i}.down", x, n, h, w)
                 skips.append((x, h, w))
         x = self._tap("mid_block.resnets.0", self._resnet("mid_block.resnets.0", x, None, tembs, n, h, w, rpb(h, w)), n, h, w)
@@ -381,8 +408,10 @@ class UNetEngine:
                 if sp.motion:
                     x = self._tap(f"up_blocks.{i}.motion_modules.{j}", self._motion(f"up_blocks.{i}.motion_modules.{j}", x, b, f, h * w), n, h, w)
             if i < nb - 1:
-                x = self._up(f"up_blocks.{i}.up", x, n, h, w)
-                h, w = 2 * h, 2 * w
+                # the target is the skip tensor now on top of the stack (unet_3d_edit_bkfill.py:544-545)
+                _, th, tw = skips[-1]
+                x = self._up(f"up_blocks.{i}.up", x, n, h, w, th, tw)
+                h, w = th, tw
                 self._tap(f"up_blocks.{i}.up", x, n, h, w)
         return x, h, w
 
@@ -402,7 +431,7 @@ class UNetEngine:
         keys|values already projected with the READER's to_k/to_v: {path: [nb, hw, 2C]}. `self` is the reference
         UNet (motion=False). latents [nb, 4, h, w]."""
         nbr, c, h, w = latents.shape
-        self.check_latent_size(h, w)
+        self.levels(h, w)
         x_in = ops.ncfhw_to_nhwc(latents.to(self.device).unsqueeze(2).contiguous(), 8, self.dtype)
         tembs = self._time_embed(torch.zeros(nbr, device=self.device))
         st = {"xattn": self.cross_attn_vectors(ehs)}
@@ -496,7 +525,7 @@ class UNetEngine:
         st = self.clip_state
         assert st is not None, "begin_clip() must run before forward()"
         b, c, f, h, w = sample.shape
-        self.check_latent_size(h, w)
+        self.levels(h, w)
         if st["bank_index"] is None or st["bank_index"].numel() != b * f:
             self.begin_clip_frames(f, b)
         t = timestep if torch.is_tensor(timestep) else torch.tensor([timestep])
@@ -587,16 +616,28 @@ class _VAEBlocks:
     def _attn(self, key, x, n, hw):
         a = self.w[key]
         C = x.shape[1]
-        t = ops.groupnorm(x, *a["gn"], n, hw, groups=self.groups, eps=1e-6)
+        # The key axis is the N of the logits GEMM and the K of P.V, and both must be multiples of 8. When hw is not (the
+        # 98 x 98 latent of a 784 x 784 image), every image's keys are read as hw + pad rows: the next image's first rows,
+        # or zero rows after the last image. The logits GEMM's column bias sets those pad logits to -inf, so the softmax
+        # gives them weight 0 exactly and P.V adds 0 x (a finite value) for them.
+        pad = -hw % 8
+        tb = torch.zeros((n * hw + pad, C), dtype=x.dtype, device=x.device) if pad else None
+        t = ops.groupnorm(x, *a["gn"], n, hw, groups=self.groups, eps=1e-6, out=None if tb is None else tb[:n * hw])
+        tk = t if tb is None else tb
         q = ops.gemm(t, a["q"][0], bias=a["q"][1])
-        k = ops.gemm(t, a["k"][0], bias=a["k"][1])
+        k = ops.gemm(tk, a["k"][0], bias=a["k"][1])
+        mask = None
+        if pad:
+            mask = torch.zeros(hw + pad, dtype=x.dtype, device=x.device)
+            mask[hw:] = float("-inf")
         out = torch.empty_like(x)
         scale = C ** -0.5
         for i in range(n):
             sl = slice(i * hw, (i + 1) * hw)
-            s = ops.gemm(q[sl], k[sl], scale=scale)                      # [hw, hw] logits
+            kl = slice(i * hw, (i + 1) * hw + pad)
+            s = ops.gemm(q[sl], k[kl], scale=scale, bias=mask)          # [hw, hw + pad] logits
             ops.softmax_rows_(s)
-            vt = ops.gemm(a["v"][0], t[sl])                              # V^T (bias folded below: rows of P sum to 1)
+            vt = ops.gemm(a["v"][0], tk[kl])                             # V^T (bias folded below: rows of P sum to 1)
             o = ops.gemm(s, vt, bias=a["v"][1])                          # P V + b_v
             ops.gemm(o, a["o"][0], out=out[sl], bias=a["o"][1], residual=x[sl])
         return out

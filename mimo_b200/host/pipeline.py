@@ -71,6 +71,14 @@ def _dedupe_images(images) -> "tuple[list, torch.Tensor]":
     return first, torch.tensor(inverse, dtype=torch.long)
 
 
+def shard_tokens(h: int, w: int, levels: int) -> int:
+    """Tokens per frame that every UNet level splits evenly: the gcd of h_l * w_l over the levels (engine.latent_levels).
+    A frame group of G GPUs cuts each motion module's tokens into G pixel shards, so G must divide it. For latents that
+    are multiples of 2^(levels - 1) this is the coarsest level's count; at 98 x 98 (784 x 784 pixels) it is 1."""
+    import math
+    return math.gcd(*(a * b for a, b in E.latent_levels(h, w, levels)))
+
+
 _POOL = None
 
 
@@ -291,14 +299,19 @@ class Pose2VideoPipeline:
         return latents * self.scheduler.init_noise_sigma
 
     def check_size(self, width: int, height: int) -> None:
-        """Width and height must be multiples of 8 x 2^(UNet levels - 1) = 64 pixels. The reference also runs other sizes
-        (run_animate.py's default is 784 x 784) through `forward_upsample_size` (unet_3d_edit_bkfill.py:430-435), which
-        this engine does not implement: say so before any work is done."""
+        """Whether the UNets' fused x2 upsampler serves every level: width and height multiples of 8 x 2^(UNet levels - 1)
+        = 64 pixels. __call__ runs other sizes too (run_animate.py's default is 784 x 784): the levels that do not double
+        exactly take the reference's `forward_upsample_size` path (unet_3d_edit_bkfill.py:430-435)."""
         m = self.vae_scale_factor << (len(self.denoising_unet.config.block_out_channels) - 1)
         if width % m or height % m:
-            raise NotImplementedError(f"width x height = {width} x {height}: both must be multiples of {m} (the "
-                                      "reference's forward_upsample_size path for other sizes is not implemented); "
-                                      f"e.g. {width // m * m or m} x {height // m * m or m}")
+            raise NotImplementedError(f"width x height = {width} x {height}: not both multiples of {m}, so some UNet up "
+                                      "steps take the forward_upsample_size path instead of the fused x2 kernel; "
+                                      f"the nearest sizes it serves are e.g. {width // m * m or m} x {height // m * m or m}")
+
+    def latent_levels(self, width: int, height: int):
+        """(h, w) of the latents at every UNet level for an image of width x height (engine.latent_levels)."""
+        return E.latent_levels(height // self.vae_scale_factor, width // self.vae_scale_factor,
+                               len(self.denoising_unet.config.block_out_channels))
 
     # ------------------------------------------------------------------------------------------------
     def preprocess(self, ref_image, pose_images, vid_bk_images, width, height, video_length, generator,
@@ -414,9 +427,8 @@ class Pose2VideoPipeline:
             from .shard import ShardPlan
             if len({len(c) for c in windows}) != 1:
                 raise NotImplementedError("context windows of different lengths cannot be sharded")
-            hmin = max(1, h >> (len(self.denoising_unet.config.block_out_channels) - 1))
-            wmin = max(1, w >> (len(self.denoising_unet.config.block_out_channels) - 1))
-            plan = ShardPlan.make(world, rank, do_cfg, len(windows), len(windows[0]), min_tokens=hmin * wmin)
+            plan = ShardPlan.make(world, rank, do_cfg, len(windows), len(windows[0]),
+                                  min_tokens=shard_tokens(h, w, len(self.denoising_unet.config.block_out_channels)))
             forced = getattr(self, "force_plan", None)  # (cfg_ways, win_ways, frame_ways): tests exercise every axis
             if forced is not None:
                 assert forced[0] * forced[1] * forced[2] == world
@@ -537,7 +549,7 @@ class Pose2VideoPipeline:
             raise NotImplementedError("eta != 0, context_batch_size != 1, interpolation_factor >= 2 and "
                                       "num_images_per_prompt != 1 are outside the reference's shipped configuration")
         dtype = self.denoising_unet.dtype
-        self.check_size(width, height)
+        self.latent_levels(width, height)  # refuses only images smaller than one latent pixel
         host = self.preprocess(ref_image, pose_images, vid_bk_images, width, height, video_length, generator, dtype)
         dev_in = {k: v.to(device, non_blocking=True) for k, v in host.items()}
         self.io_bytes["h2d"] = sum(v.numel() * v.element_size() for v in host.values())

@@ -137,6 +137,7 @@ SYMBOLS = {
     "mimo_ncfhw_to_nhwc": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP]),
     "mimo_nhwc_to_ncfhw": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP]),
     "mimo_upsample2x": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I32, _VP]),
+    "mimo_upsample_nearest": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP]),
     "mimo_softmax_rows": (C.c_int, [_VP, _I64, _I32, _I64, _I32, _VP]),
     "mimo_add": (C.c_int, [_VP, _VP, _VP, _I64, _I32, _VP]),
     "mimo_silu": (C.c_int, [_VP, _VP, _I64, _I32, _VP]),

@@ -353,6 +353,20 @@ def upsample2x(x: torch.Tensor, n: int, h: int, w: int, out: Optional[torch.Tens
     return out
 
 
+def upsample_nearest(x: torch.Tensor, n: int, h: int, w: int, oh: int, ow: int,
+                     out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """F.interpolate(mode="nearest", size=(oh, ow)) of channels-last x [n*h*w, c] -> [n*oh*ow, c], bit-identical."""
+    c = x.shape[1]
+    assert x.is_contiguous() and x.shape[0] == n * h * w
+    if out is None:
+        out = torch.empty((n * oh * ow, c), dtype=x.dtype, device=x.device)
+    assert out.is_contiguous() and out.shape == (n * oh * ow, c)
+    with _Call("upsample_nearest", 1, 0.0, float(x.element_size() * (x.numel() + out.numel()))):
+        L.check(L.load().mimo_upsample_nearest(_ptr(x), _ptr(out), n, h, w, oh, ow, c, _dt(x), _stream()),
+                "mimo_upsample_nearest")
+    return out
+
+
 def softmax_rows_(x: torch.Tensor) -> torch.Tensor:
     assert x.dim() == 2 and x.stride(1) == 1
     with _Call("softmax_rows", 1, 0.0, 2.0 * 2 * x.numel()):
