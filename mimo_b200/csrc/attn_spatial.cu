@@ -12,6 +12,13 @@
 // Q/K/V tiles arrive by 4-D TMA boxes straight out of the fused QKV activation buffer ([token, 3C] rows, head
 // slices addressed by a tensor-map dimension); head dims 40/80/160 are zero-filled up to 64-element chunks by
 // TMA's out-of-bounds handling, so no padded copies exist in HBM.
+//
+// Schedule with two MMA warpgroups, two K/V stages and registers for a second S tile (DP <= 80, kLook): a warpgroup
+// issues S(j+1) = Q K(j+1)^T and O += P(j) V(j) back to back, runs the softmax of S(j+1) while both MMAs run, and
+// rescales O once P(j) V(j) has landed. The two warpgroups take turns at issuing (named barriers 1 and 2), so one's
+// softmax runs while the other's MMAs occupy the tensor cores. Each row still computes O(j) = O(j-1) alpha(j) + P(j) V(j)
+// in the same order as the plain loop (S, softmax, rescale, P V per tile) that DP = 96 ... 144 and the one-warpgroup
+// path run.
 #include <cuda_runtime.h>
 
 #include "../../include/mimo_b200.h"
@@ -23,9 +30,10 @@
 namespace mimo {
 
 // Registers are reserved per group of 4 warps. With two MMA warpgroups (+ the TMA warp = 12 warps' worth) a thread may
-// hold 168 registers: enough for S (64) + O (d/2) below d = 160. From d = 160 on a CTA has ONE MMA warpgroup (64 query
-// rows, 8 warps' worth, up to 255 registers), so O, S and P stay in registers without spills, and the smaller Q tile
-// leaves room for a second K/V stage.
+// hold 168 registers: enough for S (64) + O (d/2) below d = 160, and up to d = 80 for the lookahead's S(j+1) (64) +
+// P(j) (32) + O (ptxas -v: 0 spills). From d = 160 on a CTA has ONE MMA warpgroup (64 query rows, 8 warps' worth, up to
+// 255 registers), so O, S and P stay in registers without spills, and the smaller Q tile leaves room for a second K/V
+// stage.
 template <int DP>
 struct AttnCfg {
   static constexpr int NCH = (DP + 63) / 64;                   // 64-column chunks of Q / K / V
@@ -36,10 +44,66 @@ struct AttnCfg {
   static constexpr int kQBytes = NCH * kQChunk;
   static constexpr int kKVStageBytes = 2 * NCH * kChunkBytes;  // K chunks then V chunks
   static constexpr int kFit = (227 * 1024 - 1024 - 256 - kQBytes) / kKVStageBytes;
-  static constexpr int KVST = kFit < 3 ? kFit : 3;             // K/V stages that fit next to Q
+  static constexpr int KVST = kFit < 4 ? kFit : 4;             // K/V stages that fit next to Q
+  // S(j+1) is loaded while stage j still feeds P(j) V(j): the lookahead needs two stages, and registers (above)
+  static constexpr bool kLook = NWG == 2 && KVST >= 2 && DP <= 80;
   static constexpr int kSmemBytes = kQBytes + KVST * kKVStageBytes + 1024 + 256;
   static_assert(KVST >= 1, "K/V tile does not fit");
 };
+
+// One online-softmax step on an S tile: row maxima over the tile's valid keys (kMask: the tile holds fewer than BKV
+// keys, the others become -inf), the new running max m, alpha = the factor for the previous O and l, l updated, and P
+// converted to the A fragments of P.V (k-step kk covers keys [16 kk, 16 kk + 16) = S fragments 2 kk, 2 kk + 1).
+// Accumulator layout (S and O alike): this thread holds rows rbase and rbase + 8; fragment j (8 columns) holds columns
+// 8 j + q2, + 1 in [4 j], [4 j + 1] (row rbase) and [4 j + 2], [4 j + 3] (row rbase + 8).
+template <bool kMask, bool kBf16>
+__device__ __forceinline__ void softmax_tile(float (&s)[BKV / 2], int valid, int q2, float scale_log2, float (&m)[2],
+                                             float (&l)[2], float (&alpha)[2], uint32_t (&pa)[BKV / 16][4]) {
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int jn = 0; jn < BKV / 8; ++jn)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      if (!kMask || 8 * jn + q2 + (e & 1) < valid)
+        mx[e >> 1] = fmaxf(mx[e >> 1], s[4 * jn + e]);
+      else
+        s[4 * jn + e] = -INFINITY;
+    }
+  float m_new[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+    mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+    m_new[r] = fmaxf(m[r], mx[r] * scale_log2);
+    alpha[r] = ex2_ftz(m[r] - m_new[r]);
+  }
+  float rowsum[2] = {0.f, 0.f};
+#pragma unroll
+  for (int kk = 0; kk < BKV / 16; ++kk)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int e = 8 * kk + 2 * i;  // i: (row, keys 0-7), (row + 8, keys 0-7), (row, keys 8-15), (row + 8, keys 8-15)
+      const int r = i & 1;
+      const float p0 = ex2_ftz(fmaf(s[e], scale_log2, -m_new[r]));
+      const float p1 = ex2_ftz(fmaf(s[e + 1], scale_log2, -m_new[r]));
+      rowsum[r] += p0 + p1;
+      pa[kk][i] = Cvt<kBf16>::pack(p0, p1);
+    }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l[r] = l[r] * alpha[r] + rowsum[r];
+    m[r] = m_new[r];
+  }
+}
+
+template <bool kBf16>
+__device__ __forceinline__ void softmax_step(float (&s)[BKV / 2], int valid, int q2, float scale_log2, float (&m)[2],
+                                             float (&l)[2], float (&alpha)[2], uint32_t (&pa)[BKV / 16][4]) {
+  if (valid < BKV)  // only the ragged last tile of the self or bank keys
+    softmax_tile<true, kBf16>(s, valid, q2, scale_log2, m, l, alpha, pa);
+  else
+    softmax_tile<false, kBf16>(s, valid, q2, scale_log2, m, l, alpha, pa);
+}
 
 template <int DP, bool kBf16>
 __global__ void __launch_bounds__(AttnCfg<DP>::kThreads, 1)
@@ -87,7 +151,8 @@ attn_spatial_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   }
   __syncthreads();
 
-  if (warp == kProd && lane == 0) {
+  if (warp == kProd) {
+    if (lane != 0) return;
     // ===================== TMA producer =====================
     mbar_expect_tx(q_full, Cfg::kQBytes);
 #pragma unroll
@@ -110,109 +175,131 @@ attn_spatial_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         tma_load_4d(sv + ch * kChunkBytes, mv, &kv_full[stage], ch * 64, h, row0, img);
       }
     }
-  } else if (warp < kProd) {
-    // ===================== MMA / softmax / epilogue =====================
-    const int wg = warp >> 2;  // query rows [64 wg, 64 wg + 64) of the tile
-    // accumulator layout (S and O alike): this thread holds rows rbase and rbase + 8; fragment j (8 columns) holds
-    // columns 8 j + q2, + 1 in [4 j], [4 j + 1] (row rbase) and [4 j + 2], [4 j + 3] (row rbase + 8)
-    const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-    const int q2 = (lane & 3) * 2;
-    const uint32_t q_addr = smem_u32(sQ) + wg * (64 * 128);
-    float o[DP / 2];
-    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
-    mbar_wait(q_full, 0);
-    for (int j = 0; j < T; ++j) {
-      const int stage = j % KVST;
-      const bool bank = j >= a.n_self_tiles;
-      const int len = bank ? a.lb : a.lq;
-      const int row0 = (bank ? j - a.n_self_tiles : j) * BKV;
-      int valid = len - row0;
-      if (valid > BKV) valid = BKV;
-      mbar_wait(&kv_full[stage], (j / KVST) & 1u);
-      const uint32_t k_addr = smem_u32(sKV + stage * Cfg::kKVStageBytes);
-      const uint32_t v_addr = k_addr + NCH * kChunkBytes;
+    return;
+  }
+  // ===================== MMA / softmax / epilogue =====================
+  const int wg = warp >> 2;  // query rows [64 wg, 64 wg + 64) of the tile
+  const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int q2 = (lane & 3) * 2;
+  const uint32_t q_addr = smem_u32(sQ) + wg * (64 * 128);
+  const float scale_log2 = a.scale_log2;
+  // keys of tile j that exist (the last self tile and the last bank tile may be ragged)
+  auto tile_valid = [&](int j) {
+    const bool bank = j >= a.n_self_tiles;
+    const int valid = (bank ? a.lb : a.lq) - (bank ? j - a.n_self_tiles : j) * BKV;
+    return valid < BKV ? valid : BKV;
+  };
+  auto kv_addr = [&](int j) { return smem_u32(sKV + (j % KVST) * Cfg::kKVStageBytes); };
+  auto wait_kv = [&](int j) { mbar_wait(&kv_full[j % KVST], (j / KVST) & 1u); };
+  auto issue_s = [&](float (&s)[BKV / 2], uint32_t k_addr) {
+#pragma unroll
+    for (int ks = 0; ks < DP / 16; ++ks) {
+      const uint32_t off = (ks & 3) * 32;
+      Wgmma<BKV, kBf16>::ss(s, make_smem_desc_sw128(q_addr + (ks >> 2) * Cfg::kQChunk + off, 16, 1024),
+                            make_smem_desc_sw128(k_addr + (ks >> 2) * kChunkBytes + off, 16, 1024), ks != 0 ? 1u : 0u);
+    }
+  };
+  float o[DP / 2];
+  auto issue_pv = [&](const uint32_t (&pa)[BKV / 16][4], uint32_t v_addr, bool first) {
+#pragma unroll
+    for (int kk = 0; kk < BKV / 16; ++kk) {
+      // B = V: MN-major, 16 keys = 2 KiB further down; 64-column chunks kChunkBytes apart
+      Wgmma<DP, kBf16>::rs(o, pa[kk], make_smem_desc_sw128(v_addr + kk * 2048, kChunkBytes, 1024),
+                           (!first || kk != 0) ? 1u : 0u);
+    }
+  };
+  auto release = [&](int j) {
+    if (lane == 0) mbar_arrive(&kv_empty[j % KVST]);
+  };
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f}, alpha[2];
+  float s[BKV / 2];
+  uint32_t pa[BKV / 16][4];
+  mbar_wait(q_full, 0);
 
-      float s[BKV / 2];
+  if constexpr (Cfg::kLook) {
+    // turns at issuing MMAs: warpgroup wg waits on barrier 1 + wg and hands over on the other's; warpgroup 1 hands
+    // the first turn to warpgroup 0 and skips its hand-over after its last turn, so every phase completes
+    const int bar_mine = 1 + wg, bar_other = 2 - wg;
+    if (wg == 1) bar_arrive(bar_other, 256);
+    wait_kv(0);
+    bar_sync(bar_mine, 256);
+    wgmma_fence();
+    issue_s(s, kv_addr(0));
+    wgmma_commit();
+    bar_arrive(bar_other, 256);
+    wgmma_wait<0>();
+    reg_fence(s);
+    softmax_step<kBf16>(s, tile_valid(0), q2, scale_log2, m, l, alpha, pa);
+    for (int j = 0; j + 1 < T; ++j) {
+      wait_kv(j + 1);
+      bar_sync(bar_mine, 256);
       wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < DP / 16; ++ks) {
-        const uint32_t off = (ks & 3) * 32;
-        Wgmma<BKV, kBf16>::ss(s, make_smem_desc_sw128(q_addr + (ks >> 2) * Cfg::kQChunk + off, 16, 1024),
-                              make_smem_desc_sw128(k_addr + (ks >> 2) * kChunkBytes + off, 16, 1024), ks != 0 ? 1u : 0u);
-      }
+      issue_s(s, kv_addr(j + 1));
       wgmma_commit();
-      wgmma_wait<0>();
+      issue_pv(pa, kv_addr(j) + NCH * kChunkBytes, j == 0);
+      wgmma_commit();
+      bar_arrive(bar_other, 256);
+      uint32_t pn[BKV / 16][4];
+      wgmma_wait<1>();
       reg_fence(s);
-
-      // row maximum over the valid keys (a row is spread over the 4 lanes of a quad)
-      float mx[2] = {-INFINITY, -INFINITY};
+      softmax_step<kBf16>(s, tile_valid(j + 1), q2, scale_log2, m, l, alpha, pn);
+      wgmma_wait<0>();
+      reg_fence(o);
+      release(j);
 #pragma unroll
-      for (int jn = 0; jn < BKV / 8; ++jn)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          if (8 * jn + q2 + (e & 1) < valid)
-            mx[e >> 1] = fmaxf(mx[e >> 1], s[4 * jn + e]);
-          else
-            s[4 * jn + e] = -INFINITY;
-        }
-      float alpha[2], m_new[2];
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-        m_new[r] = fmaxf(m[r], mx[r] * a.scale_log2);
-        alpha[r] = exp2f(m[r] - m_new[r]);
-      }
-      // probabilities -> A fragments of P.V: k-step kk covers keys [16 kk, 16 kk + 16) = S fragments 2 kk, 2 kk + 1
-      uint32_t pa[BKV / 16][4];
-      float rowsum[2] = {0.f, 0.f};
+      for (int i = 0; i < DP / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
+      // P(j+1) replaces P(j). The byte permute (= pn) reads P(j) after the wait: ptxas ends a register's life at the
+      // wgmma that reads it, and a plain copy let the softmax reuse P(j)'s registers while P(j) V(j) was still running,
+      // which ptxas answers by serializing every wgmma of the kernel.
 #pragma unroll
       for (int kk = 0; kk < BKV / 16; ++kk)
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int e = 8 * kk + 2 * i;  // i: (row, keys 0-7), (row + 8, keys 0-7), (row, keys 8-15), (row + 8, keys 8-15)
-          const int r = i & 1;
-          const float p0 = exp2f(fmaf(s[e], a.scale_log2, -m_new[r]));
-          const float p1 = exp2f(fmaf(s[e + 1], a.scale_log2, -m_new[r]));
-          rowsum[r] += p0 + p1;
-          pa[kk][i] = C::pack(p0, p1);
-        }
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        l[r] = l[r] * alpha[r] + rowsum[r];
-        m[r] = m_new[r];
-      }
+        for (int i = 0; i < 4; ++i) pa[kk][i] = __byte_perm(pa[kk][i], pn[kk][i], 0x7654);
+    }
+    // last tile: P(T-1) V(T-1) alone; warpgroup 1 keeps its turn (see above)
+    bar_sync(bar_mine, 256);
+    wgmma_fence();
+    issue_pv(pa, kv_addr(T - 1) + NCH * kChunkBytes, T == 1);
+    wgmma_commit();
+    if (wg == 0) bar_arrive(bar_other, 256);
+    wgmma_wait<0>();
+    reg_fence(o);
+    release(T - 1);
+  } else {
+    for (int j = 0; j < T; ++j) {
+      wait_kv(j);
+      wgmma_fence();
+      issue_s(s, kv_addr(j));
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(s);
+      softmax_step<kBf16>(s, tile_valid(j), q2, scale_log2, m, l, alpha, pa);
       if (j > 0) {
 #pragma unroll
         for (int i = 0; i < DP / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
       }
       wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < BKV / 16; ++kk) {
-        // B = V: MN-major, 16 keys = 2 KiB further down; 64-column chunks kChunkBytes apart
-        Wgmma<DP, kBf16>::rs(o, pa[kk], make_smem_desc_sw128(v_addr + kk * 2048, kChunkBytes, 1024),
-                             (j | kk) != 0 ? 1u : 0u);
-      }
+      issue_pv(pa, kv_addr(j) + NCH * kChunkBytes, j == 0);
       wgmma_commit();
       wgmma_wait<0>();
       reg_fence(o);
-      if (lane == 0) mbar_arrive(&kv_empty[stage]);
+      release(j);
     }
-    // epilogue: O / l -> global
+  }
+  // epilogue: O / l -> global
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
-      l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
-      const float inv_l = 1.0f / l[r];
-      const int qrow = q_tile * Cfg::QROWS + rbase + 8 * r;
-      if (qrow < a.lq) {
-        typename C::T* orow =
-            static_cast<typename C::T*>(a.out) + (static_cast<long long>(n) * a.lq + qrow) * a.ld_out + h * a.d;
+  for (int r = 0; r < 2; ++r) {
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
+    const float inv_l = 1.0f / l[r];
+    const int qrow = q_tile * Cfg::QROWS + rbase + 8 * r;
+    if (qrow < a.lq) {
+      typename C::T* orow =
+          static_cast<typename C::T*>(a.out) + (static_cast<long long>(n) * a.lq + qrow) * a.ld_out + h * a.d;
 #pragma unroll
-        for (int jn = 0; jn < DP / 8; ++jn)
-          if (8 * jn + q2 < a.d)
-            *reinterpret_cast<uint32_t*>(orow + 8 * jn + q2) = C::pack(o[4 * jn + 2 * r] * inv_l, o[4 * jn + 2 * r + 1] * inv_l);
-      }
+      for (int jn = 0; jn < DP / 8; ++jn)
+        if (8 * jn + q2 < a.d)
+          *reinterpret_cast<uint32_t*>(orow + 8 * jn + q2) = C::pack(o[4 * jn + 2 * r] * inv_l, o[4 * jn + 2 * r + 1] * inv_l);
     }
   }
 }

@@ -152,6 +152,14 @@ __device__ __forceinline__ void reg_fence(float (&d)[N]) {
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// Named barriers (id 0 is __syncthreads): `count` threads, a multiple of 32, complete one phase; bar_arrive does not wait.
+__device__ __forceinline__ void bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void bar_arrive(int id, int count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
 // Shared-memory matrix descriptor, 128-byte swizzle (tile rows are 128 B = 64 x 16-bit, 8-row / 1024-B swizzle atoms;
 // the tile base must be 1024-B aligned):
 //   [0,14) start address >> 4   [16,30) leading byte offset >> 4   [32,46) stride byte offset >> 4
@@ -171,6 +179,13 @@ __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uin
 // ------------------------------------------------------------------------------------------------
 // small numeric helpers
 // ------------------------------------------------------------------------------------------------
+// 2^x on the MUFU alone. exp2f executes the same MUFU.EX2 on the same input, plus a fix-up (a compare and two
+// multiplies) that only changes results below 2^-126, which flush to zero here.
+__device__ __forceinline__ float ex2_ftz(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
 __device__ __forceinline__ float silu_f(float x) { return __fdividef(x, 1.0f + __expf(-x)); }  // MUFU rcp, no slow path
 // exact (erf) GELU, as torch.nn.functional.gelu default
 __device__ __forceinline__ float gelu_erf_f(float x) {
