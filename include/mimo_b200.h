@@ -282,6 +282,27 @@ int mimo_cfg_ddim_step(const void* pred_uncond, const void* pred_cond, const voi
                        int64_t frame_stride, void* latents, int64_t count, float guidance, float sqrt_a_t,
                        float sqrt_1ma_t, float sqrt_a_prev, float sqrt_1ma_prev, int32_t dtype, void* stream);
 
+/* mimo_cfg_ddim_step for stochastic DDIM (eta > 0): the same update with the direction coefficient passed in, plus
+ * noise, as diffusers DDIMScheduler.step [3P] computes it with eta > 0:
+ *   x_prev = sa_p * x0 + dir_coef * e + sigma * noise,   dir_coef = sqrt(1 - abar_prev - sigma^2),
+ *   sigma = eta * sqrt((1 - abar_prev) / (1 - abar_t) * (1 - abar_t / abar_prev)).
+ * noise is [count] in `dtype` (the caller's draw, randn_tensor(model_output.shape, generator)). Each product and sum is
+ * rounded to `dtype` where the torch expression rounds it. Replaces pipeline :128-147, :421, :551-553 with eta > 0.
+ * Requirements: sigma >= 0, dir_coef >= 0. */
+int mimo_cfg_ddim_step_noise(const void* pred_uncond, const void* pred_cond, const void* counter_or_null,
+                             int64_t frame_stride, void* latents, int64_t count, float guidance, float sqrt_a_t,
+                             float sqrt_1ma_t, float sqrt_a_prev, float dir_coef, const void* noise, float sigma,
+                             int32_t dtype, void* stream);
+
+/* Latent frame interpolation (pipeline interpolate_latents, :294-334, with the methods of src/pipelines/utils.py):
+ * src [1, 4, F, h, w] -> dst [1, 4, (F-1)*k + 1, h, w] (hw = h * w): frame i goes to i*k, and k-1 frames
+ * interp(v_i, v_{i+1}, j / k) fill the gap. method 0 = linear, (1 - t) * v0 + t * v1 rounded where PyTorch rounds it
+ * (bit-identical to the torch expression on CUDA); method 1 = slerp: cos from fp32 sums over the pair's 4*hw elements in a
+ * fixed order (deterministic), |cos| > 0.9995 -> linear, else fp32 great-circle formula rounded once. The branch is taken
+ * on the device (graph-capturable). One CTA per frame pair. Requirements: F >= 2, k >= 2, src and dst distinct. */
+int mimo_interpolate_frames(const void* src, void* dst, int32_t frames, int64_t hw, int32_t k, int32_t method,
+                            int32_t dtype, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -215,13 +215,14 @@ __global__ void ew_kernel(const void* __restrict__ a, const void* __restrict__ b
   }
 }
 
-// CFG + DDIM (v-prediction, eta = 0). Every intermediate is rounded to the storage type where the reference's
-// torch expression would round it (it runs the whole update in the latents' dtype).
-template <bool kBf16>
+// CFG + DDIM (v-prediction). Every intermediate is rounded to the storage type where the reference's torch expression
+// would round it (it runs the whole update in the latents' dtype). kNoise: stochastic DDIM (eta > 0): s1a_p is then the
+// direction coefficient sqrt(1 - abar_prev - sigma^2), and sigma * noise is added last, as DDIMScheduler.step [3P] does.
+template <bool kBf16, bool kNoise>
 __global__ void cfg_ddim_kernel(const void* __restrict__ pu, const void* __restrict__ pc,
                                 const void* __restrict__ counter, long long frame_stride, int frames,
                                 void* __restrict__ lat, long long count, float g, float sa_t, float s1a_t,
-                                float sa_p, float s1a_p) {
+                                float sa_p, float s1a_p, const void* __restrict__ noise, float sigma) {
   using C = Cvt<kBf16>;
   using T = typename C::T;
   auto rnd = [](float v) { return C::to_f(C::from_f(v)); };
@@ -241,8 +242,91 @@ __global__ void cfg_ddim_kernel(const void* __restrict__ pu, const void* __restr
     const float x0 = rnd(rnd(sa_t * x) - rnd(s1a_t * v));
     const float e = rnd(rnd(sa_t * v) + rnd(s1a_t * x));
     const float dir = rnd(s1a_p * e);
-    const float prev = rnd(rnd(sa_p * x0) + dir);
+    float prev = rnd(rnd(sa_p * x0) + dir);
+    if constexpr (kNoise) prev = rnd(prev + rnd(sigma * C::to_f(static_cast<const T*>(noise)[i])));
     static_cast<T*>(lat)[i] = C::from_f(prev);
+  }
+}
+
+// Latent frame interpolation (pipeline interpolate_latents, :294-334): one CTA per frame pair (i, i + 1) of
+// src [4, F, hw] (the [1, 4, F, h, w] latents); writes dst frames i*k (a copy of frame i) and i*k + j, j = 1 .. k-1, of
+// dst [4, (F-1)*k + 1, hw]; the last CTA also copies frame F-1. Weights: t = j / k and 1 - t in double, as the reference's
+// Python floats are, then cast to fp32 as PyTorch does for a scalar operand. method 0 (linear): (1 - t) * v0 + t * v1,
+// each product rounded to the storage type, then the sum - PyTorch's rounding points for that expression. method 1
+// (slerp): |v0|^2, |v1|^2 and v0.v1 are fp32 sums in a fixed order (per-thread strided, then a fixed shuffle / shared
+// memory tree: deterministic); |cos| > 0.9995 takes the linear path, else (sin((1-t) theta) v0 + sin(t theta) v1) /
+// sin(theta) in fp32 with precise acosf / sinf, rounded once at the store.
+template <bool kBf16>
+__global__ void __launch_bounds__(256) interpolate_frames_kernel(const void* __restrict__ srcp, void* __restrict__ dstp,
+                                                                 int frames, long long hw, int k, int method) {
+  using C = Cvt<kBf16>;
+  using T = typename C::T;
+  auto rnd = [](float v) { return C::to_f(C::from_f(v)); };
+  const T* src = static_cast<const T*>(srcp);
+  T* dst = static_cast<T*>(dstp);
+  const int i = blockIdx.x;
+  const long long fo = static_cast<long long>(frames - 1) * k + 1;
+  bool slerp = method == 1;
+  float theta = 0.f, sin_theta = 1.f;
+  if (slerp) {
+    __shared__ float red[3][8];
+    float s00 = 0.f, s11 = 0.f, s01 = 0.f;
+    for (int c = 0; c < 4; ++c) {
+      const T* a = src + (static_cast<long long>(c) * frames + i) * hw;
+      for (long long p = threadIdx.x; p < hw; p += blockDim.x) {
+        const float x0 = C::to_f(a[p]), x1 = C::to_f(a[p + hw]);
+        s00 = fmaf(x0, x0, s00);
+        s11 = fmaf(x1, x1, s11);
+        s01 = fmaf(x0, x1, s01);
+      }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+      s00 += __shfl_xor_sync(0xffffffffu, s00, o);
+      s11 += __shfl_xor_sync(0xffffffffu, s11, o);
+      s01 += __shfl_xor_sync(0xffffffffu, s01, o);
+    }
+    if ((threadIdx.x & 31) == 0) {
+      red[0][threadIdx.x >> 5] = s00;
+      red[1][threadIdx.x >> 5] = s11;
+      red[2][threadIdx.x >> 5] = s01;
+    }
+    __syncthreads();
+    s00 = s11 = s01 = 0.f;
+    for (int w = 0; w < static_cast<int>(blockDim.x >> 5); ++w) {
+      s00 += red[0][w];
+      s11 += red[1][w];
+      s01 += red[2][w];
+    }
+    const float cosv = __fdiv_rn(s01, __fmul_rn(sqrtf(s00), sqrtf(s11)));
+    // the branch is taken on the device (no host sync): the call stays capturable in a graph. NaN (a zero frame)
+    // fails the test and propagates, as in the reference.
+    slerp = !(fabsf(cosv) > 0.9995f);
+    if (slerp) {
+      theta = acosf(cosv);
+      sin_theta = sinf(theta);
+    }
+  }
+  for (int c = 0; c < 4; ++c) {
+    const T* a = src + (static_cast<long long>(c) * frames + i) * hw;
+    T* o = dst + (static_cast<long long>(c) * fo + static_cast<long long>(i) * k) * hw;
+    for (long long p = threadIdx.x; p < hw; p += blockDim.x) {
+      const T v0 = a[p], v1 = a[p + hw];
+      const float x0 = C::to_f(v0), x1 = C::to_f(v1);
+      o[p] = v0;
+      for (int j = 1; j < k; ++j) {
+        const double t = static_cast<double>(j) / k;
+        const float wa = static_cast<float>(1.0 - t), wb = static_cast<float>(t);
+        float y;
+        if (slerp) {
+          y = __fdiv_rn(__fadd_rn(__fmul_rn(sinf(__fmul_rn(wa, theta)), x0), __fmul_rn(sinf(__fmul_rn(wb, theta)), x1)),
+                        sin_theta);
+        } else {
+          y = rnd(__fmul_rn(wa, x0)) + rnd(__fmul_rn(wb, x1));
+        }
+        o[static_cast<long long>(j) * hw + p] = C::from_f(y);
+      }
+      if (i == frames - 2) o[static_cast<long long>(k) * hw + p] = v1;
+    }
   }
 }
 
@@ -432,13 +516,62 @@ extern "C" int mimo_cfg_ddim_step(const void* pred_uncond, const void* pred_cond
     frames = static_cast<int>(count / (4 * frame_stride));
   }
   if (dtype == MIMO_BF16)
-    cfg_ddim_kernel<true><<<ew_grid(count, 256), 256, 0, st>>>(pred_uncond, pred_cond, counter_or_null, frame_stride,
-                                                              frames, latents, count, guidance, sqrt_a_t,
-                                                              sqrt_1ma_t, sqrt_a_prev, sqrt_1ma_prev);
+    cfg_ddim_kernel<true, false><<<ew_grid(count, 256), 256, 0, st>>>(pred_uncond, pred_cond, counter_or_null,
+                                                                     frame_stride, frames, latents, count, guidance,
+                                                                     sqrt_a_t, sqrt_1ma_t, sqrt_a_prev, sqrt_1ma_prev,
+                                                                     nullptr, 0.f);
   else
-    cfg_ddim_kernel<false><<<ew_grid(count, 256), 256, 0, st>>>(pred_uncond, pred_cond, counter_or_null,
-                                                               frame_stride, frames, latents, count, guidance,
-                                                               sqrt_a_t, sqrt_1ma_t, sqrt_a_prev, sqrt_1ma_prev);
+    cfg_ddim_kernel<false, false><<<ew_grid(count, 256), 256, 0, st>>>(pred_uncond, pred_cond, counter_or_null,
+                                                                      frame_stride, frames, latents, count, guidance,
+                                                                      sqrt_a_t, sqrt_1ma_t, sqrt_a_prev, sqrt_1ma_prev,
+                                                                      nullptr, 0.f);
   MIMO_CHECK_LAUNCH("cfg_ddim launch");
+  return MIMO_OK;
+}
+
+extern "C" int mimo_cfg_ddim_step_noise(const void* pred_uncond, const void* pred_cond, const void* counter_or_null,
+                                        int64_t frame_stride, void* latents, int64_t count, float guidance,
+                                        float sqrt_a_t, float sqrt_1ma_t, float sqrt_a_prev, float dir_coef,
+                                        const void* noise, float sigma, int32_t dtype, void* stream) {
+  if (!pred_uncond || !pred_cond || !latents || !noise || count <= 0)
+    return set_error(MIMO_ERR_ARG, "mimo_cfg_ddim_step_noise: null pointer or count <= 0");
+  if (dtype != MIMO_F16 && dtype != MIMO_BF16) return set_error(MIMO_ERR_ARG, "mimo_cfg_ddim_step_noise: bad dtype");
+  if (!(sigma >= 0.f) || !(dir_coef >= 0.f))  // also refuses NaN (sqrt of a negative variance)
+    return set_error(MIMO_ERR_ARG, "mimo_cfg_ddim_step_noise: sigma and dir_coef must be >= 0");
+  int frames = 1;
+  if (counter_or_null) {
+    if (frame_stride <= 0 || count % (4 * frame_stride))
+      return set_error(MIMO_ERR_ARG, "mimo_cfg_ddim_step_noise: bad frame_stride");
+    frames = static_cast<int>(count / (4 * frame_stride));
+  }
+  if (int rc = ensure_device()) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (dtype == MIMO_BF16)
+    cfg_ddim_kernel<true, true><<<ew_grid(count, 256), 256, 0, st>>>(pred_uncond, pred_cond, counter_or_null,
+                                                                    frame_stride, frames, latents, count, guidance,
+                                                                    sqrt_a_t, sqrt_1ma_t, sqrt_a_prev, dir_coef,
+                                                                    noise, sigma);
+  else
+    cfg_ddim_kernel<false, true><<<ew_grid(count, 256), 256, 0, st>>>(pred_uncond, pred_cond, counter_or_null,
+                                                                     frame_stride, frames, latents, count, guidance,
+                                                                     sqrt_a_t, sqrt_1ma_t, sqrt_a_prev, dir_coef,
+                                                                     noise, sigma);
+  MIMO_CHECK_LAUNCH("cfg_ddim_noise launch");
+  return MIMO_OK;
+}
+
+extern "C" int mimo_interpolate_frames(const void* src, void* dst, int32_t frames, int64_t hw, int32_t k, int32_t method,
+                                       int32_t dtype, void* stream) {
+  if (!src || !dst || src == dst) return set_error(MIMO_ERR_ARG, "mimo_interpolate_frames: null or aliased pointers");
+  if (frames < 2 || hw <= 0 || k < 2 || (method != 0 && method != 1))
+    return set_error(MIMO_ERR_ARG, "mimo_interpolate_frames: need frames >= 2, hw > 0, k >= 2, method 0 or 1");
+  if (dtype != MIMO_F16 && dtype != MIMO_BF16) return set_error(MIMO_ERR_ARG, "mimo_interpolate_frames: bad dtype");
+  if (int rc = ensure_device()) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (dtype == MIMO_BF16)
+    interpolate_frames_kernel<true><<<frames - 1, 256, 0, st>>>(src, dst, frames, hw, k, method);
+  else
+    interpolate_frames_kernel<false><<<frames - 1, 256, 0, st>>>(src, dst, frames, hw, k, method);
+  MIMO_CHECK_LAUNCH("interpolate_frames launch");
   return MIMO_OK;
 }

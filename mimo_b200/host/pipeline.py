@@ -4,7 +4,8 @@
 What stays as in the reference: PIL pre-processing semantics, CLIP through the HF module the caller passes, the CPU
 generator noise (prepare_latents :149-183), context windows (:492-510), CFG (:545-549) and DDIM (:551-553) maths.
 What changes is where the arithmetic runs: reference_unet / pose_guider / denoising_unet / VAE are engine objects
-behind the C ABI; the CFG + DDIM update is one fused kernel; all frames are decoded in one batched VAE pass.
+behind the C ABI; the CFG + DDIM update (also with eta > 0) is one fused kernel, latent frame interpolation another; the
+frames are decoded in batched VAE passes (one pass up to DECODE_PIXELS_PER_PASS output pixels).
 
 __call__ = preprocess() [host: PIL -> pinned tensors]  ->  H2D  ->  sample_tensors() [device]  ->  D2H.
 """
@@ -275,10 +276,28 @@ class Pose2VideoPipeline:
             self._vae_engines = (E.VAEEncoderEngine(sd, self.device, dt), E.VAEDecoderEngine(sd, self.device, dt))
         return self._vae_engines
 
-    def decode_latents_device(self, latents: torch.Tensor) -> torch.Tensor:
-        """[1, 4, F, h, w] -> device tensor [1, 3, F, H, W] in [0, 1] (pipeline :113-123), one batched engine pass."""
+    # Output pixels one batched VAE decode pass may cover: 48 frames at 768 x 768, the largest clip the benchmark decodes on
+    # one GPU (its widest activation, 128 channels at full resolution, is then 3.6 G elements, ~7 GB in 16 bits). Every
+    # clip up to that size keeps one pass; longer ones (e.g. an interpolated 784 x 784 clip) decode in chunks of frames.
+    DECODE_PIXELS_PER_PASS = 48 * 768 * 768
+
+    def decode_latents_device(self, latents: torch.Tensor, frames_per_pass: Optional[int] = None) -> torch.Tensor:
+        """[1, 4, F, h, w] -> device tensor [1, 3, F, H, W] in [0, 1] (pipeline :113-123): batched engine passes of at
+        most `frames_per_pass` frames (default: DECODE_PIXELS_PER_PASS worth). The decoder's arithmetic is per image,
+        so the chunked result is byte-identical to one pass."""
         z = (1 / 0.18215 * latents)[0].permute(1, 0, 2, 3).contiguous()
-        frames = self._vae()[1].decode(z)  # [F, 3, H, W]
+        dec = self._vae()[1]
+        n, s = z.shape[0], self.vae_scale_factor
+        per = frames_per_pass or max(1, self.DECODE_PIXELS_PER_PASS // (z.shape[2] * s * z.shape[3] * s))
+        if n <= per:
+            frames = dec.decode(z)  # [F, 3, H, W]
+        else:
+            first = dec.decode(z[:per])
+            frames = torch.empty((n,) + tuple(first.shape[1:]), dtype=first.dtype, device=first.device)
+            frames[:per] = first
+            del first
+            for i in range(per, n, per):
+                frames[i:i + per] = dec.decode(z[i:i + per])
         video = frames.permute(1, 0, 2, 3).unsqueeze(0)
         return (video / 2 + 0.5).clamp(0, 1)
 
@@ -314,10 +333,26 @@ class Pose2VideoPipeline:
                                len(self.denoising_unet.config.block_out_channels))
 
     # ------------------------------------------------------------------------------------------------
+    def _draw_noise(self, width, height, video_length, dtype, generator, num_inference_steps: int, eta: float,
+                    pinned: bool):
+        """The clip's random draws in the reference's order: the initial latents (prepare_latents), then, when eta > 0
+        and a generator is given, one randn_tensor(model_output.shape) per DDIM step (DDIMScheduler.step [3P], also at
+        the last step), stacked in one (pinned) tensor [steps, 1, 4, F, h, w]. Without a generator the step noise is
+        drawn on the device inside the loop, as randn_tensor does."""
+        latents = self.prepare_latents(1, 4, width, height, video_length, dtype, "cpu", generator)
+        if not (eta > 0 and generator is not None and num_inference_steps > 0):
+            return latents, None
+        shape = tuple(latents.shape)
+        noise = torch.empty((num_inference_steps,) + shape, dtype=dtype, pin_memory=pinned)
+        for i in range(num_inference_steps):
+            noise[i] = _randn_tensor(shape, generator, torch.device("cpu"), dtype)
+        return latents, noise
+
     def preprocess(self, ref_image, pose_images, vid_bk_images, width, height, video_length, generator,
-                   dtype) -> Dict[str, torch.Tensor]:
+                   dtype, num_inference_steps: int = 0, eta: float = 0.0) -> Dict[str, torch.Tensor]:
         """Host side of __call__: PIL -> pinned CPU tensors (what the reference does at pipeline :379-381, :409-418,
-        :424-426, :435-437, :446-453 before anything touches the device)."""
+        :424-426, :435-437, :446-453 before anything touches the device). With eta > 0 and a generator, the per-step
+        DDIM noise is drawn here too, right after the initial latents, as "step_noise"."""
         pinned = torch.cuda.is_available()
         pin = lambda t: t.contiguous().pin_memory() if pinned else t.contiguous()
         bks = list(vid_bk_images)
@@ -325,7 +360,8 @@ class Pose2VideoPipeline:
             raise ValueError(f"video_length={video_length} but {len(pose_images)} pose images and {len(bks)} background "
                              "images were passed (pipeline :435-453 indexes both per frame)")
         # the noise draw (CPU generator, target dtype: ~10 ms of one core for a 24-frame clip) runs beside the image staging
-        noise = _pool().submit(self.prepare_latents, 1, 4, width, height, video_length, dtype, "cpu", generator)
+        noise = _pool().submit(self._draw_noise, width, height, video_length, dtype, generator, num_inference_steps, eta,
+                               pinned)
         try:
             # identical background frames are converted, copied and encoded once; every frame is written straight into
             # its pinned staging tensor (stage_frames_u8: same bytes as pil_to_uint8, without the intermediate copies)
@@ -338,18 +374,45 @@ class Pose2VideoPipeline:
                 "pose_u8": stage_frames_u8(list(pose_images), height, width, pinned),  # [F, H, W, 3]
             }
         finally:
-            latents = noise.result()  # also on an error above: the generator must not be left in use by a worker
+            latents, step_noise = noise.result()  # also on an error above: the generator must not be left in use by a worker
         out["latents"] = pin(latents)
+        if step_noise is not None:
+            out["step_noise"] = step_noise
         return out
+
+    @staticmethod
+    def _interpolation_method(interpolation_factor: int, video_length: int) -> Optional[int]:
+        """The mimo_interpolate_frames method for interpolation_factor (None: no interpolation, k <= 1 as in the
+        reference). Checked before any work: the reference only fails after the whole denoising loop."""
+        if interpolation_factor is None or interpolation_factor < 2:
+            return None
+        from .interpolation import get_tensor_interpolation_method, kernel_method
+        method = kernel_method(get_tensor_interpolation_method())
+        if video_length < 2:
+            raise ValueError(f"interpolation_factor={interpolation_factor} needs at least 2 frames to interpolate "
+                             f"between, got video_length={video_length}")
+        return method
 
     @torch.no_grad()
     def sample_tensors(self, inp: Dict[str, torch.Tensor], num_inference_steps: int, guidance_scale: float,
                        context_schedule="uniform", context_frames=24, context_stride=1, context_overlap=4,
-                       callback=None, callback_steps=1, decode: bool = True) -> Dict[str, torch.Tensor]:
-        """Device side: everything in `inp` already lives in HBM; returns device tensors."""
+                       callback=None, callback_steps=1, decode: bool = True, eta: float = 0.0,
+                       interpolation_factor: int = 1) -> Dict[str, torch.Tensor]:
+        """Device side: everything in `inp` already lives in HBM; returns device tensors. eta > 0: stochastic DDIM with
+        inp["step_noise"] [steps, 1, 4, F, h, w] (preprocess draws it from the generator), or, without it, noise drawn
+        on the device at every step. interpolation_factor k >= 2: the registered interpolation method inserts k-1
+        frames between neighbours before the decode; out["latents"] stays the denoised clip."""
         device = self.device
         dtype = self.denoising_unet.dtype
         do_cfg = guidance_scale > 1.0
+        if eta < 0:
+            raise ValueError(f"eta={eta}: DDIM's eta is >= 0 (0 deterministic, 1 DDPM-like)")
+        interp = self._interpolation_method(interpolation_factor, inp["latents"].shape[2])
+        step_noise = inp.get("step_noise") if eta > 0 else None
+        if step_noise is not None and (step_noise.shape[0] < num_inference_steps
+                                       or tuple(step_noise.shape[1:]) != tuple(inp["latents"].shape)):
+            raise ValueError(f"step_noise {tuple(step_noise.shape)} does not hold {num_inference_steps} draws of "
+                             f"{tuple(inp['latents'].shape)}")
         ev = lambda: torch.cuda.Event(enable_timing=True)
         marks = [("start", ev())]
         marks[0][1].record()
@@ -498,13 +561,18 @@ class Pose2VideoPipeline:
                         noise_pred[:, :, c] = noise_pred[:, :, c] + pred  # :540-542
                         counter[c] = counter[c] + 1
             co = self.scheduler.step_coefficients(t)
-            if do_cfg:
-                ops.cfg_ddim_step(noise_pred[0], noise_pred[1], latents, guidance_scale, *co, counter=counter,
-                                  frame_stride=h * w)
+            # the reference divides the window sums by `counter` only inside its guidance branch (pipeline :545-549):
+            # without CFG, frames that two windows cover keep the SUM of both predictions - mirrored, not repaired
+            pc, g_, cnt = (noise_pred[1], guidance_scale, counter) if do_cfg else (noise_pred[0], 1.0, None)
+            if eta > 0:
+                # DDIMScheduler.step [3P] draws its noise at every step, also the last one (sigma = 0 there)
+                dir_c, sigma = self.scheduler.noise_coefficients(t, eta)
+                noise = (step_noise[i] if step_noise is not None
+                         else torch.randn(tuple(latents.shape), device=device, dtype=dtype))
+                ops.cfg_ddim_step_noise(noise_pred[0], pc, latents, g_, *co[:3], dir_c, noise, sigma, counter=cnt,
+                                        frame_stride=h * w)
             else:
-                # the reference divides the window sums by `counter` only inside its guidance branch (pipeline :545-549):
-                # without CFG, frames that two windows cover keep the SUM of both predictions - mirrored, not repaired
-                ops.cfg_ddim_step(noise_pred[0], noise_pred[0], latents, 1.0, *co, counter=None, frame_stride=h * w)
+                ops.cfg_ddim_step(noise_pred[0], pc, latents, g_, *co, counter=cnt, frame_stride=h * w)
             # the reference's inner `for i in range(num_context_batches)` (pipeline :503-510) shadows the step index: its
             # callback test (:556-561) and the index it passes see the LAST CONTEXT BATCH's index, at every step
             i_ref = len(windows) - 1
@@ -515,15 +583,20 @@ class Pose2VideoPipeline:
         writer.clear()
         out = {"latents": latents}
         if decode:
-            if world > 1 and F_ % world == 0:
-                fl = F_ // world
-                loc = self.decode_latents_device(latents[:, :, rank * fl:(rank + 1) * fl])  # [1, 3, fl, H, W]
+            vid_lat = latents
+            if interp is not None:  # pipeline :566-567: the frames to decode, (F - 1) * k + 1 of them
+                vid_lat = ops.interpolate_frames(latents, interpolation_factor, interp)
+                mark("interpolate")
+            Fv = vid_lat.shape[2]
+            if world > 1 and Fv % world == 0:
+                fl = Fv // world
+                loc = self.decode_latents_device(vid_lat[:, :, rank * fl:(rank + 1) * fl])  # [1, 3, fl, H, W]
                 parts = torch.empty((world * loc.shape[0],) + tuple(loc.shape[1:]), dtype=loc.dtype, device=device)
                 dist.all_gather_into_tensor(parts, loc.contiguous(), group=group)
                 out["videos"] = parts.view((world,) + tuple(loc.shape)).permute(1, 2, 0, 3, 4, 5).reshape(
-                    1, 3, F_, loc.shape[-2], loc.shape[-1])
+                    1, 3, Fv, loc.shape[-2], loc.shape[-1])
             else:
-                out["videos"] = self.decode_latents_device(latents)
+                out["videos"] = self.decode_latents_device(vid_lat)
             mark("vae_decode")
         self._marks = marks
         self.last_latents = latents
@@ -545,16 +618,21 @@ class Pose2VideoPipeline:
         device = self.device
         if device.type != "cuda":
             raise MimoError("Pose2VideoPipeline needs its models on a CUDA (sm_90a) device: no CPU fallback")
-        if eta != 0.0 or context_batch_size != 1 or interpolation_factor not in (0, 1) or num_images_per_prompt != 1:
-            raise NotImplementedError("eta != 0, context_batch_size != 1, interpolation_factor >= 2 and "
-                                      "num_images_per_prompt != 1 are outside the reference's shipped configuration")
+        if context_batch_size != 1 or num_images_per_prompt != 1:
+            raise NotImplementedError("context_batch_size != 1 and num_images_per_prompt != 1 are outside the "
+                                      "reference's shipped configuration")
+        if eta < 0:
+            raise ValueError(f"eta={eta}: DDIM's eta is >= 0 (0 deterministic, 1 DDPM-like)")
+        self._interpolation_method(interpolation_factor, video_length)  # before any work is done
         dtype = self.denoising_unet.dtype
         self.latent_levels(width, height)  # refuses only images smaller than one latent pixel
-        host = self.preprocess(ref_image, pose_images, vid_bk_images, width, height, video_length, generator, dtype)
+        host = self.preprocess(ref_image, pose_images, vid_bk_images, width, height, video_length, generator, dtype,
+                               num_inference_steps, eta)
         dev_in = {k: v.to(device, non_blocking=True) for k, v in host.items()}
         self.io_bytes["h2d"] = sum(v.numel() * v.element_size() for v in host.values())
         out = self.sample_tensors(dev_in, num_inference_steps, guidance_scale, context_schedule, context_frames,
-                                  context_stride, context_overlap, callback, callback_steps)
+                                  context_stride, context_overlap, callback, callback_steps, eta=eta,
+                                  interpolation_factor=interpolation_factor)
         vid = out["videos"].float()  # :124-126 "always cast to float32": exact, and 20 ms cheaper here than on one host core
         host_vid = torch.empty(vid.shape, dtype=torch.float32, pin_memory=True)
         host_vid.copy_(vid, non_blocking=True)  # one D2H of the finished clip, into pinned memory

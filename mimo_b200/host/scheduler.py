@@ -72,24 +72,37 @@ class DDIMScheduler:
     def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, eta: float = 0.0,
              use_clipped_model_output: bool = False, generator=None, variance_noise=None, return_dict: bool = True,
              **unused):
-        """diffusers DDIMScheduler.step [3P] for v-prediction, eta = 0 (pipeline :551-553): tensor in, tensor out, in
-        the dtype / on the device of `sample`. The engine's own sampler uses the fused kernel (step_coefficients);
+        """diffusers DDIMScheduler.step [3P] for v-prediction (pipeline :128-147, :551-553): tensor in, tensor out, in
+        the dtype / on the device of `sample`. eta > 0 adds sigma * noise, the noise being `variance_noise` or drawn by
+        randn_tensor(model_output.shape, generator, dtype=model_output.dtype) - at every call, also at the last step
+        where sigma = 0. The engine's own sampler uses the fused kernels (step_coefficients / noise_coefficients);
         this method exists so that the reference's unmodified pipeline file runs over this scheduler."""
         if self.num_inference_steps is None:
             raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating "
                              "the scheduler")
-        if eta != 0.0 or use_clipped_model_output or variance_noise is not None:
-            raise NotImplementedError("eta != 0 / clipped model output / variance noise are outside the reference's "
-                                      "shipped configuration")
+        if use_clipped_model_output:
+            raise NotImplementedError("use_clipped_model_output is outside the reference's shipped configuration")
+        if eta == 0.0 and variance_noise is not None:
+            raise NotImplementedError("variance_noise at eta = 0 is outside the reference's shipped configuration")
         t = int(timestep)
-        prev_t = t - self.config.num_train_timesteps // self.num_inference_steps
-        a_t = self.alphas_cumprod[t]
-        a_p = self.alphas_cumprod[prev_t] if prev_t >= 0 else self.final_alpha_cumprod
+        a_t, a_p = self._alphas(t)
         b_t = 1 - a_t
         x0 = (a_t ** 0.5) * sample - (b_t ** 0.5) * model_output
         eps = (a_t ** 0.5) * model_output + (b_t ** 0.5) * sample
-        direction = (1 - a_p) ** 0.5 * eps  # std_dev_t = 0 at eta = 0
-        prev = a_p ** 0.5 * x0 + direction
+        if eta > 0:
+            if variance_noise is not None and generator is not None:
+                raise ValueError("Cannot pass both generator and variance_noise. Please make sure that either "
+                                 "`generator` or `variance_noise` stays `None`.")
+            std_dev_t = eta * self._variance(a_t, a_p) ** 0.5
+            direction = self._direction(a_p, std_dev_t) * eps
+            prev = a_p ** 0.5 * x0 + direction
+            if variance_noise is None:
+                from .pipeline import _randn_tensor
+                variance_noise = _randn_tensor(model_output.shape, generator, model_output.device, model_output.dtype)
+            prev = prev + std_dev_t * variance_noise
+        else:
+            direction = (1 - a_p) ** 0.5 * eps  # std_dev_t = 0 at eta = 0
+            prev = a_p ** 0.5 * x0 + direction
         if not return_dict:
             return (prev,)
         return SimpleNamespace(prev_sample=prev, pred_original_sample=x0)
@@ -101,3 +114,28 @@ class DDIMScheduler:
         a_t = self.alphas_cumprod[t]
         a_p = self.alphas_cumprod[prev_t] if prev_t >= 0 else self.final_alpha_cumprod
         return float(a_t ** 0.5), float((1 - a_t) ** 0.5), float(a_p ** 0.5), float((1 - a_p) ** 0.5)
+
+    def _alphas(self, t: int):
+        prev_t = t - self.config.num_train_timesteps // self.num_inference_steps
+        a_p = self.alphas_cumprod[prev_t] if prev_t >= 0 else self.final_alpha_cumprod
+        return self.alphas_cumprod[t], a_p
+
+    @staticmethod
+    def _variance(a_t, a_p):
+        """DDIMScheduler._get_variance [3P]: (1 - abar_prev) / (1 - abar_t) * (1 - abar_t / abar_prev), fp32."""
+        return ((1 - a_p) / (1 - a_t)) * (1 - a_t / a_p)
+
+    @staticmethod
+    def _direction(a_p, std_dev_t):
+        """sqrt(1 - abar_prev - sigma^2) in fp32, the radicand clamped at 0. At eta = 1 on a zero-terminal-SNR schedule
+        (rescale_betas_zero_snr, abar = 0 at t = 999) the first step's radicand is exactly 0 in real arithmetic, and
+        fp32 rounding can make it -1 ulp (at 20 and 25 steps): diffusers then returns NaN latents for the whole clip;
+        here the square root is of 0, the exact value. Everywhere else the result is diffusers' to the bit."""
+        return (1 - a_p - std_dev_t ** 2).clamp(min=0) ** 0.5
+
+    def noise_coefficients(self, t: int, eta: float):
+        """(sqrt(1 - abar_prev - sigma^2), sigma) with sigma = eta * sqrt(variance): the direction coefficient and the
+        noise scale of a stochastic DDIM step (eta > 0), in the fp32 tensor arithmetic of DDIMScheduler.step [3P]."""
+        a_t, a_p = self._alphas(t)
+        std_dev_t = eta * self._variance(a_t, a_p) ** 0.5
+        return float(self._direction(a_p, std_dev_t)), float(std_dev_t)

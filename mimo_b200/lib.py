@@ -144,6 +144,8 @@ SYMBOLS = {
     "mimo_quick_gelu": (C.c_int, [_VP, _VP, _I64, _I32, _VP]),
     "mimo_composite_frame": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP, C.c_double, _VP, _I64, _VP]),
     "mimo_cfg_ddim_step": (C.c_int, [_VP, _VP, _VP, _I64, _VP, _I64, _F, _F, _F, _F, _F, _I32, _VP]),
+    "mimo_cfg_ddim_step_noise": (C.c_int, [_VP, _VP, _VP, _I64, _VP, _I64, _F, _F, _F, _F, _F, _VP, _F, _I32, _VP]),
+    "mimo_interpolate_frames": (C.c_int, [_VP, _VP, _I32, _I64, _I32, _I32, _I32, _VP]),
 }
 # test hook, not part of the public header
 _DEBUG_SYMBOLS = {"mimo_debug_pdl": (C.c_int, [C.c_int]), "mimo_debug_splitk": (C.c_int, [C.c_int]),

@@ -428,6 +428,38 @@ def cfg_ddim_step(pred_uncond: torch.Tensor, pred_cond: torch.Tensor, latents: t
     return latents
 
 
+def cfg_ddim_step_noise(pred_uncond: torch.Tensor, pred_cond: torch.Tensor, latents: torch.Tensor, guidance: float,
+                        sqrt_a_t: float, sqrt_1ma_t: float, sqrt_a_prev: float, dir_coef: float, noise: torch.Tensor,
+                        sigma: float, *, counter: Optional[torch.Tensor] = None, frame_stride: int = 0) -> torch.Tensor:
+    """cfg_ddim_step for eta > 0: direction coefficient `dir_coef` = sqrt(1 - abar_prev - sigma^2), plus sigma * noise."""
+    assert pred_uncond.is_contiguous() and pred_cond.is_contiguous() and latents.is_contiguous()
+    assert noise.is_contiguous() and noise.numel() == latents.numel() and noise.dtype == latents.dtype
+    with _Call("cfg_ddim", 1, 0.0, 2.0 * 5 * latents.numel()):
+        L.check(L.load().mimo_cfg_ddim_step_noise(_ptr(pred_uncond), _ptr(pred_cond), _ptr(counter), int(frame_stride),
+                                                  _ptr(latents), latents.numel(), float(guidance), float(sqrt_a_t),
+                                                  float(sqrt_1ma_t), float(sqrt_a_prev), float(dir_coef), _ptr(noise),
+                                                  float(sigma), _dt(latents), _stream()), "mimo_cfg_ddim_step_noise")
+    return latents
+
+
+INTERP_LINEAR, INTERP_SLERP = 0, 1
+
+
+def interpolate_frames(latents: torch.Tensor, k: int, method: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """[1, 4, F, h, w] -> [1, 4, (F-1)*k + 1, h, w]: k-1 interpolated frames between each pair of neighbours
+    (pipeline interpolate_latents); method INTERP_LINEAR or INTERP_SLERP."""
+    b, c, f, h, w = latents.shape
+    assert b == 1 and c == 4 and latents.is_contiguous()
+    shape = (1, 4, (f - 1) * k + 1, h, w)
+    if out is None:
+        out = torch.empty(shape, dtype=latents.dtype, device=latents.device)
+    assert out.is_contiguous() and tuple(out.shape) == shape and out.dtype == latents.dtype
+    with _Call("interpolate_frames", 1, 0.0, float(latents.element_size() * (2 * latents.numel() + out.numel()))):
+        L.check(L.load().mimo_interpolate_frames(_ptr(latents), _ptr(out), f, h * w, k, method, _dt(latents), _stream()),
+                "mimo_interpolate_frames")
+    return out
+
+
 # ------------------------------------------------------------------------------------------------
 # weight packing (host side, once per model load)
 # ------------------------------------------------------------------------------------------------

@@ -1,27 +1,10 @@
 """reference: src/pipelines/utils.py — the latent-interpolation method registry the pipeline file imports
-(pipeline_pose2vid_long_edit_bkfill_roiclip.py:27, :327). Dead code at interpolation_factor = 1 (the shipped value),
-kept so that the reference's unmodified pipeline file imports over this overlay."""
-import torch
-
-_method = None
-
-
-def get_tensor_interpolation_method():
-    return _method
-
-
-def set_tensor_interpolation_method(is_slerp):
-    global _method
-    _method = slerp if is_slerp else linear
-
-
-def linear(v1, v2, t):
-    return (1.0 - t) * v1 + t * v2  # this evaluation order: bit-identical to the reference's
-
-
-def slerp(v0: torch.Tensor, v1: torch.Tensor, t: float, DOT_THRESHOLD: float = 0.9995) -> torch.Tensor:
-    cos = (v0 / v0.norm() * (v1 / v1.norm())).sum()
-    if cos.abs() > DOT_THRESHOLD:  # nearly parallel: the great-circle formula is ill-conditioned
-        return (1.0 - t) * v0 + t * v1
-    theta = cos.acos()
-    return (torch.sin((1.0 - t) * theta) * v0 + torch.sin(t * theta) * v1) / torch.sin(theta)
+(pipeline_pose2vid_long_edit_bkfill_roiclip.py:27, :327). It lives in mimo_b200/host/interpolation.py, where the
+engine's sampler reads it for interpolation_factor >= 2; this module re-exports it so that the reference's unmodified
+pipeline file and run scripts register the method the same way."""
+from mimo_b200.host.interpolation import (  # noqa: F401
+    get_tensor_interpolation_method,
+    linear,
+    set_tensor_interpolation_method,
+    slerp,
+)
