@@ -41,7 +41,8 @@ const char* mimo_last_error(void);
 /* 0 if device `dev` is sm_90; MIMO_ERR_DEVICE otherwise (also when there is no CUDA device at all). */
 int mimo_device_check(int dev);
 /* sizeof() of the parameter structs as compiled into the library (0 epilogue, 1 gemm, 2 conv3x3, 3 groupnorm,
- * 4 attn, 5 attn_temporal, 6 exchange): lets a binding verify its struct mirrors before the first call. */
+ * 4 attn, 5 attn_temporal, 6 exchange, 7 cfg_multistep): lets a binding verify its struct mirrors before the first
+ * call. */
 int mimo_abi_sizeof(int which);
 
 /* Fused epilogue shared by GEMM and conv:  out = act((acc + bias[c] + rowvec[row / rows_per_group][c]
@@ -293,6 +294,33 @@ int mimo_cfg_ddim_step_noise(const void* pred_uncond, const void* pred_cond, con
                              int64_t frame_stride, void* latents, int64_t count, float guidance, float sqrt_a_t,
                              float sqrt_1ma_t, float sqrt_a_prev, float dir_coef, const void* noise, float sigma,
                              int32_t dtype, void* stream);
+
+/* Classifier-free guidance + one step of a multistep / sigma-space solver (DPM-Solver++ orders 1-3, Euler,
+ * Euler-ancestral; v-prediction), one pass. Per element, with v the guided prediction exactly as in mimo_cfg_ddim_step
+ * (same roundings: the reference's torch ops at pipeline :545-549):
+ *   m  = rnd(a * x + b * v)                                   the solver's model quantity, written to hist_out
+ *   x' = c_x * x + c_m * m + c_1 * h1 + c_2 * h2 + c_n * noise  in fp32, rounded once at the store into latents
+ * h1 / h2 are the m of the previous two steps. The host computes the eight scalars per step (host/scheduler.py:
+ * multistep_coefficients). Replaces pipeline :519-521, :545-553 with a DPMSolverMultistepScheduler,
+ * EulerDiscreteScheduler or EulerAncestralDiscreteScheduler [3P]. */
+typedef struct {
+  const void* pred_uncond; /* [count]                                                                      */
+  const void* pred_cond;   /* [count]                                                                      */
+  const void* counter;     /* [F] window count per frame (as mimo_cfg_ddim_step), or NULL                  */
+  int64_t frame_stride;    /* h * w: latents are [1, 4, F, h, w]; needed with counter                      */
+  void* latents;           /* [count], updated in place                                                    */
+  int64_t count;
+  void* hist_out;          /* [count] receives m; may alias h2 (each element is read before it is written)  */
+  const void* h1;          /* [count] or NULL (then c_1 must be 0)                                         */
+  const void* h2;          /* [count] or NULL (then c_2 must be 0)                                         */
+  const void* noise;       /* [count] or NULL (then c_n must be 0)                                         */
+  float guidance;
+  float a, b;              /* m = a * x + b * v                                                            */
+  float c_x, c_m, c_1, c_2, c_n;
+  int32_t dtype;
+} mimo_cfg_multistep_params;
+/* Requirements: finite scalars; hist_out distinct from latents, pred_*, h1 and noise. Graph-capturable. */
+int mimo_cfg_multistep(const mimo_cfg_multistep_params* p, void* stream);
 
 /* Latent frame interpolation (pipeline interpolate_latents, :294-334, with the methods of src/pipelines/utils.py):
  * src [1, 4, F, h, w] -> dst [1, 4, (F-1)*k + 1, h, w] (hw = h * w): frame i goes to i*k, and k-1 frames

@@ -1,5 +1,8 @@
-// Layout converters, im2col gather, add / SiLU, and the fused CFG + DDIM update. All single coalesced passes.
+// Layout converters, im2col gather, add / SiLU, and the fused CFG + DDIM / multistep updates. All single coalesced
+// passes.
 #include <cuda_runtime.h>
+
+#include <cmath>
 
 #include "../../include/mimo_b200.h"
 #include "host_util.h"
@@ -245,6 +248,44 @@ __global__ void cfg_ddim_kernel(const void* __restrict__ pu, const void* __restr
     float prev = rnd(rnd(sa_p * x0) + dir);
     if constexpr (kNoise) prev = rnd(prev + rnd(sigma * C::to_f(static_cast<const T*>(noise)[i])));
     static_cast<T*>(lat)[i] = C::from_f(prev);
+  }
+}
+
+// CFG + one multistep / sigma-space solver step (mimo_cfg_multistep). The guidance lines are cfg_ddim_kernel's, with its
+// roundings; m is rounded to the storage type (it is stored as history), the update is fp32 and rounded once. hist_out
+// may alias h2: h2[i] is read before hist_out[i] is written, by the same thread, so neither pointer is __restrict__.
+template <bool kBf16>
+__global__ void cfg_multistep_kernel(const mimo_cfg_multistep_params p, int frames) {
+  using C = Cvt<kBf16>;
+  using T = typename C::T;
+  auto rnd = [](float v) { return C::to_f(C::from_f(v)); };
+  const T* __restrict__ pu = static_cast<const T*>(p.pred_uncond);
+  const T* __restrict__ pc = static_cast<const T*>(p.pred_cond);
+  const T* __restrict__ cnt = static_cast<const T*>(p.counter);
+  const T* __restrict__ h1 = static_cast<const T*>(p.h1);
+  const T* __restrict__ nz = static_cast<const T*>(p.noise);
+  const T* h2 = static_cast<const T*>(p.h2);
+  T* hist = static_cast<T*>(p.hist_out);
+  T* __restrict__ lat = static_cast<T*>(p.latents);
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < p.count;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    float u = C::to_f(pu[i]);
+    float c = C::to_f(pc[i]);
+    if (cnt) {
+      const float n = C::to_f(cnt[(i / p.frame_stride) % frames]);
+      u = rnd(u / n);
+      c = rnd(c / n);
+    }
+    const float v = rnd(u + rnd(p.guidance * rnd(c - u)));
+    const float x = C::to_f(lat[i]);
+    const T mt = C::from_f(fmaf(p.a, x, p.b * v));
+    const float m = C::to_f(mt);
+    float acc = fmaf(p.c_x, x, p.c_m * m);
+    if (h1) acc = fmaf(p.c_1, C::to_f(h1[i]), acc);
+    if (h2) acc = fmaf(p.c_2, C::to_f(h2[i]), acc);
+    if (nz) acc = fmaf(p.c_n, C::to_f(nz[i]), acc);
+    hist[i] = mt;
+    lat[i] = C::from_f(acc);
   }
 }
 
@@ -557,6 +598,35 @@ extern "C" int mimo_cfg_ddim_step_noise(const void* pred_uncond, const void* pre
                                                                      sqrt_a_t, sqrt_1ma_t, sqrt_a_prev, dir_coef,
                                                                      noise, sigma);
   MIMO_CHECK_LAUNCH("cfg_ddim_noise launch");
+  return MIMO_OK;
+}
+
+extern "C" int mimo_cfg_multistep(const mimo_cfg_multistep_params* p, void* stream) {
+  if (!p || !p->pred_uncond || !p->pred_cond || !p->latents || !p->hist_out)
+    return set_error(MIMO_ERR_ARG, "mimo_cfg_multistep: null pointer");
+  if (p->count <= 0) return set_error(MIMO_ERR_ARG, "mimo_cfg_multistep: count <= 0");
+  if (p->dtype != MIMO_F16 && p->dtype != MIMO_BF16) return set_error(MIMO_ERR_ARG, "mimo_cfg_multistep: bad dtype");
+  const float sc[8] = {p->guidance, p->a, p->b, p->c_x, p->c_m, p->c_1, p->c_2, p->c_n};
+  for (float s : sc)
+    if (!std::isfinite(s)) return set_error(MIMO_ERR_ARG, "mimo_cfg_multistep: non-finite coefficient");
+  if ((!p->h1 && p->c_1 != 0.f) || (!p->h2 && p->c_2 != 0.f) || (!p->noise && p->c_n != 0.f))
+    return set_error(MIMO_ERR_ARG, "mimo_cfg_multistep: null h1 / h2 / noise with a non-zero coefficient");
+  const void* h = p->hist_out;
+  if (h == p->latents || h == p->pred_uncond || h == p->pred_cond || h == p->h1 || h == p->noise)
+    return set_error(MIMO_ERR_ARG, "mimo_cfg_multistep: hist_out aliases latents, pred_uncond, pred_cond, h1 or noise");
+  int frames = 1;
+  if (p->counter) {
+    if (p->frame_stride <= 0 || p->count % (4 * p->frame_stride))
+      return set_error(MIMO_ERR_ARG, "mimo_cfg_multistep: bad frame_stride");
+    frames = static_cast<int>(p->count / (4 * p->frame_stride));
+  }
+  if (int rc = ensure_device()) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (p->dtype == MIMO_BF16)
+    cfg_multistep_kernel<true><<<ew_grid(p->count, 256), 256, 0, st>>>(*p, frames);
+  else
+    cfg_multistep_kernel<false><<<ew_grid(p->count, 256), 256, 0, st>>>(*p, frames);
+  MIMO_CHECK_LAUNCH("cfg_multistep launch");
   return MIMO_OK;
 }
 

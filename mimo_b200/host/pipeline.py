@@ -2,9 +2,10 @@
 36-80 constructor, :338-363 __call__ signature, :573-578 output), driving the sm_90a engine.
 
 What stays as in the reference: PIL pre-processing semantics, CLIP through the HF module the caller passes, the CPU
-generator noise (prepare_latents :149-183), context windows (:492-510), CFG (:545-549) and DDIM (:551-553) maths.
+generator noise (prepare_latents :149-183), context windows (:492-510), CFG (:545-549) and scheduler (:551-553) maths.
 What changes is where the arithmetic runs: reference_unet / pose_guider / denoising_unet / VAE are engine objects
-behind the C ABI; the CFG + DDIM update (also with eta > 0) is one fused kernel, latent frame interpolation another; the
+behind the C ABI; the CFG + DDIM update (also with eta > 0) is one fused kernel, the CFG + DPM-Solver++ / Euler /
+Euler-ancestral update another (host/scheduler.py: engine_scheduler), latent frame interpolation a third; the
 frames are decoded in batched VAE passes (one pass up to DECODE_PIXELS_PER_PASS output pixels).
 
 __call__ = preprocess() [host: PIL -> pinned tensors]  ->  H2D  ->  sample_tensors() [device]  ->  D2H.
@@ -305,7 +306,9 @@ class Pose2VideoPipeline:
         return self.decode_latents_device(latents).cpu().float().numpy()  # :124-126
 
     def prepare_latents(self, batch_size, num_channels_latents, width, height, video_length, dtype, device, generator,
-                        latents=None):
+                        latents=None, scheduler=None):
+        """pipeline :149-183; `scheduler` (default self.scheduler) gives init_noise_sigma: a float, or a 0-dim fp32
+        tensor for Euler, whose multiply keeps the latents' dtype as the reference's does."""
         shape = (batch_size, num_channels_latents, video_length, height // self.vae_scale_factor,
                  width // self.vae_scale_factor)
         if isinstance(generator, list) and len(generator) != batch_size:
@@ -315,7 +318,7 @@ class Pose2VideoPipeline:
             latents = _randn_tensor(shape, generator, torch.device(device), dtype)
         else:
             latents = latents.to(device)  # pipeline :179
-        return latents * self.scheduler.init_noise_sigma
+        return latents * (scheduler if scheduler is not None else self.scheduler).init_noise_sigma
 
     def check_size(self, width: int, height: int) -> None:
         """Whether the UNets' fused x2 upsampler serves every level: width and height multiples of 8 x 2^(UNet levels - 1)
@@ -333,14 +336,23 @@ class Pose2VideoPipeline:
                                len(self.denoising_unet.config.block_out_channels))
 
     # ------------------------------------------------------------------------------------------------
+    @staticmethod
+    def _step_draws(sched, eta: float) -> bool:
+        """Whether every step of `sched` consumes one randn_tensor(model_output.shape) draw: DDIM with eta > 0
+        (DDIMScheduler.step [3P]) and Euler-ancestral; eta reaches DDIM only (prepare_extra_step_kwargs, :128-147)."""
+        from .scheduler import DDIMScheduler
+        return eta > 0 if isinstance(sched, DDIMScheduler) else sched.draws_noise
+
     def _draw_noise(self, width, height, video_length, dtype, generator, num_inference_steps: int, eta: float,
-                    pinned: bool):
-        """The clip's random draws in the reference's order: the initial latents (prepare_latents), then, when eta > 0
-        and a generator is given, one randn_tensor(model_output.shape) per DDIM step (DDIMScheduler.step [3P], also at
-        the last step), stacked in one (pinned) tensor [steps, 1, 4, F, h, w]. Without a generator the step noise is
-        drawn on the device inside the loop, as randn_tensor does."""
-        latents = self.prepare_latents(1, 4, width, height, video_length, dtype, "cpu", generator)
-        if not (eta > 0 and generator is not None and num_inference_steps > 0):
+                    pinned: bool, sched=None):
+        """The clip's random draws in the reference's order: the initial latents (prepare_latents, scaled by `sched`'s
+        init_noise_sigma), then, for schedulers whose steps consume a draw (_step_draws) and with a generator, one
+        randn_tensor(model_output.shape) per step (also at the last step), stacked in one (pinned) tensor
+        [steps, 1, 4, F, h, w]. Without a generator the step noise is drawn on the device inside the loop, as
+        randn_tensor does."""
+        sched = sched if sched is not None else self.scheduler
+        latents = self.prepare_latents(1, 4, width, height, video_length, dtype, "cpu", generator, scheduler=sched)
+        if not (self._step_draws(sched, eta) and generator is not None and num_inference_steps > 0):
             return latents, None
         shape = tuple(latents.shape)
         noise = torch.empty((num_inference_steps,) + shape, dtype=dtype, pin_memory=pinned)
@@ -351,8 +363,12 @@ class Pose2VideoPipeline:
     def preprocess(self, ref_image, pose_images, vid_bk_images, width, height, video_length, generator,
                    dtype, num_inference_steps: int = 0, eta: float = 0.0) -> Dict[str, torch.Tensor]:
         """Host side of __call__: PIL -> pinned CPU tensors (what the reference does at pipeline :379-381, :409-418,
-        :424-426, :435-437, :446-453 before anything touches the device). With eta > 0 and a generator, the per-step
-        DDIM noise is drawn here too, right after the initial latents, as "step_noise"."""
+        :424-426, :435-437, :446-453 before anything touches the device). With a generator, the per-step noise of DDIM
+        with eta > 0 or of Euler-ancestral is drawn here too, right after the initial latents, as "step_noise"."""
+        from .scheduler import engine_scheduler
+        sched = engine_scheduler(self.scheduler)
+        if num_inference_steps > 0:
+            sched.set_timesteps(num_inference_steps, device="cpu")  # init_noise_sigma may depend on the table
         pinned = torch.cuda.is_available()
         pin = lambda t: t.contiguous().pin_memory() if pinned else t.contiguous()
         bks = list(vid_bk_images)
@@ -361,7 +377,7 @@ class Pose2VideoPipeline:
                              "images were passed (pipeline :435-453 indexes both per frame)")
         # the noise draw (CPU generator, target dtype: ~10 ms of one core for a 24-frame clip) runs beside the image staging
         noise = _pool().submit(self._draw_noise, width, height, video_length, dtype, generator, num_inference_steps, eta,
-                               pinned)
+                               pinned, sched)
         try:
             # identical background frames are converted, copied and encoded once; every frame is written straight into
             # its pinned staging tensor (stage_frames_u8: same bytes as pil_to_uint8, without the intermediate copies)
@@ -401,14 +417,21 @@ class Pose2VideoPipeline:
         """Device side: everything in `inp` already lives in HBM; returns device tensors. eta > 0: stochastic DDIM with
         inp["step_noise"] [steps, 1, 4, F, h, w] (preprocess draws it from the generator), or, without it, noise drawn
         on the device at every step. interpolation_factor k >= 2: the registered interpolation method inserts k-1
-        frames between neighbours before the decode; out["latents"] stays the denoised clip."""
+        frames between neighbours before the decode; out["latents"] stays the denoised clip.
+        The scheduler is engine_scheduler(self.scheduler): DDIM runs mimo_cfg_ddim_step(_noise), DPM-Solver++, Euler and
+        Euler-ancestral one mimo_cfg_multistep per step (Euler-ancestral with inp["step_noise"] or device draws, as
+        eta > 0 does)."""
+        from .scheduler import DDIMScheduler, engine_scheduler
         device = self.device
         dtype = self.denoising_unet.dtype
         do_cfg = guidance_scale > 1.0
         if eta < 0:
             raise ValueError(f"eta={eta}: DDIM's eta is >= 0 (0 deterministic, 1 DDPM-like)")
         interp = self._interpolation_method(interpolation_factor, inp["latents"].shape[2])
-        step_noise = inp.get("step_noise") if eta > 0 else None
+        sched = engine_scheduler(self.scheduler)
+        ddim = isinstance(sched, DDIMScheduler)
+        draws = self._step_draws(sched, eta)
+        step_noise = inp.get("step_noise") if draws else None
         if step_noise is not None and (step_noise.shape[0] < num_inference_steps
                                        or tuple(step_noise.shape[1:]) != tuple(inp["latents"].shape)):
             raise ValueError(f"step_noise {tuple(step_noise.shape)} does not hold {num_inference_steps} draws of "
@@ -422,8 +445,8 @@ class Pose2VideoPipeline:
             e.record()
             marks.append((name, e))
 
-        self.scheduler.set_timesteps(num_inference_steps, device="cpu")
-        timesteps = [int(t) for t in self.scheduler.timesteps]
+        sched.set_timesteps(num_inference_steps, device="cpu")
+        timesteps = [t.item() for t in sched.timesteps]  # DDIM / DPM-Solver++: int; Euler: fp32 values
 
         emb = self._clip().image_embeds(inp["clip_pixels"]).to(dtype)  # :378-385
         ehs = emb.unsqueeze(1)
@@ -535,13 +558,20 @@ class Pose2VideoPipeline:
             if den.xchg is not None:
                 den._graphs.clear()  # graphs captured with exchange nodes must not serve an un-sharded run
             den.xchg = None
+        # multistep solvers: the model quantity m of the last two steps, slot i % 2 written at step i (every rank of a
+        # sharded run holds the whole clip's latents and keeps its own identical ring)
+        ring = None if ddim else torch.empty((2,) + tuple(latents.shape), dtype=dtype, device=device)
         for i, t in enumerate(timesteps):
+            # scale_model_input (pipeline :519-521): the reference's own expression `x / s` with s a 0-dim fp32 tensor
+            # for Euler; the identity for DDIM and DPM-Solver++
+            s_in = None if ddim else sched.model_input_scale(i)
+            lat_src = latents if s_in is None else latents / s_in
             if plan:
                 par = getattr(xw, "parity", 0)  # alternates across steps AND clips
                 xw.parity = par ^ 1
                 stage = stages[par]
                 for j, (c, cl, bk_c, pose_in) in enumerate(win_inputs):
-                    lat_in = torch.cat([latents[:, :, cl], bk_c], dim=1).repeat(nb, 1, 1, 1, 1)
+                    lat_in = torch.cat([lat_src[:, :, cl], bk_c], dim=1).repeat(nb, 1, 1, 1, 1)
                     stage[j].copy_(den.forward(lat_in, t, pose_in).reshape(-1))
                 xw.pull(2, ("S0", "S1")[par], gathered.view(-1, gcols), 1, 1, stage.numel() // gcols, gcols)
                 noise_pred = torch.zeros((rep, 4, F_, h, w), device=device, dtype=dtype)
@@ -553,25 +583,35 @@ class Pose2VideoPipeline:
                     noise_pred = torch.zeros((rep, 4, F_, h, w), device=device, dtype=dtype)
                     counter = torch.zeros((F_,), device=device, dtype=dtype)
                 for c, cl, bk_c, pose_in in win_inputs:
-                    lat_in = torch.cat([latents[:, :, cl], bk_c], dim=1).repeat(rep, 1, 1, 1, 1)
+                    lat_in = torch.cat([lat_src[:, :, cl], bk_c], dim=1).repeat(rep, 1, 1, 1, 1)
                     pred = den.forward(lat_in, t, pose_in)
                     if single:
                         noise_pred, counter = pred, None
                     else:
                         noise_pred[:, :, c] = noise_pred[:, :, c] + pred  # :540-542
                         counter[c] = counter[c] + 1
-            co = self.scheduler.step_coefficients(t)
             # the reference divides the window sums by `counter` only inside its guidance branch (pipeline :545-549):
             # without CFG, frames that two windows cover keep the SUM of both predictions - mirrored, not repaired
             pc, g_, cnt = (noise_pred[1], guidance_scale, counter) if do_cfg else (noise_pred[0], 1.0, None)
-            if eta > 0:
+            if not ddim:
+                co = sched.multistep_coefficients(i)
+                noise = None
+                if draws:  # Euler-ancestral: one draw per step, also at the last one (sigma_up = 0 there)
+                    noise = (step_noise[i] if step_noise is not None
+                             else torch.randn(tuple(latents.shape), device=device, dtype=dtype))
+                ops.cfg_multistep(noise_pred[0], pc, latents, g_, co, ring[i % 2],
+                                  h1=ring[(i - 1) % 2] if co[4] != 0 else None, h2=ring[i % 2] if co[5] != 0 else None,
+                                  noise=noise if co[6] != 0 else None, counter=cnt, frame_stride=h * w)
+            elif eta > 0:
+                co = sched.step_coefficients(t)
                 # DDIMScheduler.step [3P] draws its noise at every step, also the last one (sigma = 0 there)
-                dir_c, sigma = self.scheduler.noise_coefficients(t, eta)
+                dir_c, sigma = sched.noise_coefficients(t, eta)
                 noise = (step_noise[i] if step_noise is not None
                          else torch.randn(tuple(latents.shape), device=device, dtype=dtype))
                 ops.cfg_ddim_step_noise(noise_pred[0], pc, latents, g_, *co[:3], dir_c, noise, sigma, counter=cnt,
                                         frame_stride=h * w)
             else:
+                co = sched.step_coefficients(t)
                 ops.cfg_ddim_step(noise_pred[0], pc, latents, g_, *co, counter=cnt, frame_stride=h * w)
             # the reference's inner `for i in range(num_context_batches)` (pipeline :503-510) shadows the step index: its
             # callback test (:556-561) and the index it passes see the LAST CONTEXT BATCH's index, at every step
@@ -626,6 +666,8 @@ class Pose2VideoPipeline:
         self._interpolation_method(interpolation_factor, video_length)  # before any work is done
         dtype = self.denoising_unet.dtype
         self.latent_levels(width, height)  # refuses only images smaller than one latent pixel
+        from .scheduler import engine_scheduler
+        engine_scheduler(self.scheduler)  # refuses LMS, PNDM and unknown schedulers before any work
         host = self.preprocess(ref_image, pose_images, vid_bk_images, width, height, video_length, generator, dtype,
                                num_inference_steps, eta)
         dev_in = {k: v.to(device, non_blocking=True) for k, v in host.items()}

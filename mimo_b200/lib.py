@@ -112,6 +112,17 @@ class ExchangeParams(C.Structure):
     ]
 
 
+class CfgMultistepParams(C.Structure):
+    _fields_ = [
+        ("pred_uncond", C.c_void_p), ("pred_cond", C.c_void_p), ("counter", C.c_void_p), ("frame_stride", C.c_int64),
+        ("latents", C.c_void_p), ("count", C.c_int64),
+        ("hist_out", C.c_void_p), ("h1", C.c_void_p), ("h2", C.c_void_p), ("noise", C.c_void_p),
+        ("guidance", C.c_float), ("a", C.c_float), ("b", C.c_float),
+        ("c_x", C.c_float), ("c_m", C.c_float), ("c_1", C.c_float), ("c_2", C.c_float), ("c_n", C.c_float),
+        ("dtype", C.c_int32),
+    ]
+
+
 # every symbol include/mimo_b200.h declares: name -> (restype, argtypes)
 _VP, _I32, _I64, _F = C.c_void_p, C.c_int32, C.c_int64, C.c_float
 SYMBOLS = {
@@ -146,6 +157,7 @@ SYMBOLS = {
     "mimo_cfg_ddim_step": (C.c_int, [_VP, _VP, _VP, _I64, _VP, _I64, _F, _F, _F, _F, _F, _I32, _VP]),
     "mimo_cfg_ddim_step_noise": (C.c_int, [_VP, _VP, _VP, _I64, _VP, _I64, _F, _F, _F, _F, _F, _VP, _F, _I32, _VP]),
     "mimo_interpolate_frames": (C.c_int, [_VP, _VP, _I32, _I64, _I32, _I32, _I32, _VP]),
+    "mimo_cfg_multistep": (C.c_int, [C.POINTER(CfgMultistepParams), _VP]),
 }
 # test hook, not part of the public header
 _DEBUG_SYMBOLS = {"mimo_debug_pdl": (C.c_int, [C.c_int]), "mimo_debug_splitk": (C.c_int, [C.c_int]),
@@ -170,7 +182,7 @@ def load() -> C.CDLL:
         fn.restype = res
         fn.argtypes = args
     for which, st in enumerate((Epilogue, GemmParams, Conv3x3Params, GroupNormParams, AttnParams, AttnTemporalParams,
-                             ExchangeParams)):
+                             ExchangeParams, CfgMultistepParams)):
         if lib.mimo_abi_sizeof(which) != C.sizeof(st):
             raise MimoError(f"ABI mismatch: {st.__name__} is {C.sizeof(st)} bytes in lib.py but "
                             f"{lib.mimo_abi_sizeof(which)} in {LIB_PATH.name}; rebuild the library")

@@ -442,6 +442,29 @@ def cfg_ddim_step_noise(pred_uncond: torch.Tensor, pred_cond: torch.Tensor, late
     return latents
 
 
+def cfg_multistep(pred_uncond: torch.Tensor, pred_cond: torch.Tensor, latents: torch.Tensor, guidance: float,
+                  coefficients, hist_out: torch.Tensor, *, h1: Optional[torch.Tensor] = None,
+                  h2: Optional[torch.Tensor] = None, noise: Optional[torch.Tensor] = None,
+                  counter: Optional[torch.Tensor] = None, frame_stride: int = 0) -> torch.Tensor:
+    """In-place multistep solver update of `latents` (DPM-Solver++, Euler, Euler-ancestral) from the two CFG halves:
+    coefficients = (a, b, c_x, c_m, c_1, c_2, c_n) of the scheduler's multistep_coefficients(i); m = a x + b v goes to
+    `hist_out` (which may be `h2`). A None h1 / h2 / noise is a zero term."""
+    a, b, cx, cm, c1, c2, cn = (float(c) for c in coefficients)
+    for t in (pred_uncond, pred_cond, latents, hist_out) + tuple(x for x in (h1, h2, noise) if x is not None):
+        assert t.is_contiguous() and t.dtype == latents.dtype
+    for t in (pred_uncond, pred_cond, hist_out) + tuple(x for x in (h1, h2, noise) if x is not None):
+        assert t.numel() == latents.numel()
+    p = L.CfgMultistepParams(pred_uncond=_ptr(pred_uncond), pred_cond=_ptr(pred_cond), counter=_ptr(counter),
+                             frame_stride=int(frame_stride), latents=_ptr(latents), count=latents.numel(),
+                             hist_out=_ptr(hist_out), h1=_ptr(h1), h2=_ptr(h2), noise=_ptr(noise),
+                             guidance=float(guidance), a=a, b=b, c_x=cx, c_m=cm, c_1=c1, c_2=c2, c_n=cn,
+                             dtype=_dt(latents))
+    n_in = 3 + sum(x is not None for x in (h1, h2, noise))
+    with _Call("cfg_multistep", 1, 0.0, float(latents.element_size() * (n_in + 2) * latents.numel())):
+        L.check(L.load().mimo_cfg_multistep(C.byref(p), _stream()), "mimo_cfg_multistep")
+    return latents
+
+
 INTERP_LINEAR, INTERP_SLERP = 0, 1
 
 
