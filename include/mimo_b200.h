@@ -41,8 +41,8 @@ const char* mimo_last_error(void);
 /* 0 if device `dev` is sm_90; MIMO_ERR_DEVICE otherwise (also when there is no CUDA device at all). */
 int mimo_device_check(int dev);
 /* sizeof() of the parameter structs as compiled into the library (0 epilogue, 1 gemm, 2 conv3x3, 3 groupnorm,
- * 4 attn, 5 attn_temporal, 6 exchange, 7 cfg_multistep): lets a binding verify its struct mirrors before the first
- * call. */
+ * 4 attn, 5 attn_temporal, 6 exchange, 7 cfg_multistep, 8 groupnorm_window): lets a binding verify its struct mirrors
+ * before the first call. */
 int mimo_abi_sizeof(int which);
 
 /* Fused epilogue shared by GEMM and conv:  out = act((acc + bias[c] + rowvec[row / rows_per_group][c]
@@ -147,6 +147,40 @@ typedef struct {
 int mimo_groupnorm(const mimo_groupnorm_params* p, void* stream);
 /* bytes of `stats` workspace mimo_groupnorm needs for these sizes (pointers in *p are ignored); < 0 on bad sizes */
 int64_t mimo_groupnorm_workspace_bytes(const mimo_groupnorm_params* p);
+
+/* GroupNorm with statistics over a whole window of frames: torch.nn.GroupNorm applied to [b, C, f, h, w], which the
+ * reference builds for ResnetBlock3D norm1 / norm2 and conv_norm_out when use_inflated_groupnorm is False
+ * (src/models/resnet.py:155-163, 185-192; unet_3d_edit_bkfill.py:236-247). x is [samples, frames, hw, c0 (+ c1)]
+ * channels-last (image = sample * frames + frame); every sample gets one mean / variance per group over all frames.
+ * Deterministic and shard-invariant: a statistics pass writes a partial table with one record per (frame, sample),
+ * frame-major, so the tables of consecutive frame slices (e.g. the ranks of a frame-sharded window) concatenate into the
+ * table of the whole window; the normalisation pass adds the records in an order fixed by frame and slab index only.
+ *   mimo_groupnorm_window          both passes on x (x holds the whole window: table_frames is ignored)
+ *   mimo_groupnorm_window_partials writes the `frames` records of x's frames into table (gamma/beta/out/stats unused)
+ *   mimo_groupnorm_window_apply    normalises x's frames from a table of table_frames >= frames records
+ * Same channel rules and SiLU / two-source concat as mimo_groupnorm. All three are graph-capturable. */
+typedef struct {
+  const void* x0;
+  int32_t c0;
+  const void* x1; /* NULL if single source */
+  int32_t c1;
+  const void* gamma;
+  const void* beta;    /* [c0 + c1] */
+  void* out;           /* [samples, frames, hw, c0 + c1] */
+  float* table;        /* partial table, 16-byte aligned */
+  int64_t table_bytes; /* size of `table`: >= mimo_groupnorm_window_table_bytes per frames it holds */
+  float* stats;        /* scratch of samples * groups * 2 floats (apply / one call), contents irrelevant */
+  int32_t samples, frames, table_frames, hw, groups;
+  float eps;
+  int32_t silu;
+  int32_t dtype;
+} mimo_groupnorm_window_params;
+int mimo_groupnorm_window(const mimo_groupnorm_window_params* p, void* stream);
+int mimo_groupnorm_window_partials(const mimo_groupnorm_window_params* p, void* stream);
+int mimo_groupnorm_window_apply(const mimo_groupnorm_window_params* p, void* stream);
+/* bytes of the partial table of x's `frames` frames (pointers and table_frames ignored); < 0 on bad sizes. The table of
+ * a window sharded into G equal frame slices is G times the slice's. */
+int64_t mimo_groupnorm_window_table_bytes(const mimo_groupnorm_window_params* p);
 
 /* LayerNorm over the last dim; optional additive per-frame vector AFTER the affine (the motion module's
  * sinusoidal positional encoding): out[r] = LN(x[r]) * gamma + beta + pe[pe_frame_offset + (r / rows_per_frame) % frames]

@@ -106,6 +106,7 @@ extern "C" int mimo_abi_sizeof(int which) {
     case 5: return static_cast<int>(sizeof(mimo_attn_temporal_params));
     case 6: return static_cast<int>(sizeof(mimo_exchange_params));
     case 7: return static_cast<int>(sizeof(mimo_cfg_multistep_params));
+    case 8: return static_cast<int>(sizeof(mimo_groupnorm_window_params));
   }
   return -1;
 }

@@ -2,6 +2,7 @@
 // 128-bit loads/stores, fp32 statistics, each thread owns a fixed 8-channel vector so gamma/beta/mean/rstd
 // are loaded once and the loop over pixels is pure streaming.
 #include <cuda_runtime.h>
+#include <stdio.h>
 
 #include "../../include/mimo_b200.h"
 #include "host_util.h"
@@ -27,7 +28,7 @@ struct GnArgs {
   const void* gamma;
   const void* beta;
   void* out;
-  float* part;  // [n][bpi][groups][2] = (sum, sumsq) of x - K_g per slab
+  float* part;  // [n][bpi][groups][2] = (sum, sumsq) of x - K_g per slab; window mode: the partial table (below)
   int c0, c1, C, hw, groups, cpg;
   int vecs;  // C / 8
   int P;     // pixels processed side by side by one block
@@ -35,6 +36,10 @@ struct GnArgs {
   int bpi;   // slabs per image
   float eps;
   int silu;
+  // window mode only: image n = sample * frames + frame; statistics per sample over every frame of the window
+  int frames, samples;
+  long long rec;       // floats per (frame, sample) record of the partial table
+  const float* stats;  // [samples][groups][2] = (mean, rstd)
 };
 
 template <bool kBf16>
@@ -61,8 +66,9 @@ __device__ __forceinline__ float gn_shift(const GnArgs& a, int n, int g) {
 
 constexpr int kGnMaxThreads = 320;
 
-// pass 1: per-(image, slab, group) sum and sum of squares
-template <bool kBf16>
+// pass 1: per-(image, slab, group) sum and sum of squares. kWindow: the image is frame k of sample s, and the block
+// writes slab row 1 + blockIdx.x of record (k, s); the first slab's block also writes the record's K_g row.
+template <bool kBf16, bool kWindow = false>
 __global__ void __launch_bounds__(kGnMaxThreads) gn_stats_kernel(GnArgs a) {
   using C = Cvt<kBf16>;
   __shared__ float4 s_red[kGnMaxThreads];  // per-thread (sumA, sqA, sumB, sqB)
@@ -121,50 +127,29 @@ __global__ void __launch_bounds__(kGnMaxThreads) gn_stats_kernel(GnArgs a) {
         q += as_a ? r.y : r.w;
       }
     }
-    float* dst = a.part + ((static_cast<long long>(n) * a.bpi + blockIdx.x) * a.groups + g) * 2;
-    dst[0] = s;
-    dst[1] = q;
+    if constexpr (kWindow) {
+      const int smp = n / a.frames, k = n - smp * a.frames;
+      float* rec = a.part + (static_cast<long long>(k) * a.samples + smp) * a.rec;
+      float* dst = rec + (static_cast<long long>(1 + blockIdx.x) * a.groups + g) * 2;
+      dst[0] = s;
+      dst[1] = q;
+      if (blockIdx.x == 0) {
+        rec[2 * g] = gn_shift<kBf16>(a, n, g);
+        rec[2 * g + 1] = 0.f;
+      }
+    } else {
+      float* dst = a.part + ((static_cast<long long>(n) * a.bpi + blockIdx.x) * a.groups + g) * 2;
+      dst[0] = s;
+      dst[1] = q;
+    }
   }
 }
 
-// pass 2: image statistics from the slab partials (fixed order), then normalise + affine (+ SiLU)
+// normalise + affine (+ SiLU) of image n's slab blockIdx.x, with the per-group mean / rstd in shared memory
 template <bool kBf16>
-__global__ void __launch_bounds__(kGnMaxThreads) gn_apply_kernel(GnArgs a) {
+__device__ __forceinline__ void gn_normalise(const GnArgs& a, int n, const float* s_mean, const float* s_rstd) {
   using C = Cvt<kBf16>;
-  __shared__ float s_tot[4][128];
-  __shared__ float s_mean[64], s_rstd[64];
-  pdl_launch_dependents();
-  pdl_wait();
-  const int n = blockIdx.y;
   const int tid = threadIdx.x;
-  const int g2 = a.groups * 2;
-  {
-    // K_g first (the same thread adds the shifted mean below): the load overlaps the partial sums
-    for (int g = tid; g < a.groups; g += blockDim.x) s_mean[g] = gn_shift<kBf16>(a, n, g);
-    const int parts = a.bpi >= 16 ? 4 : 1;  // a function of the shape only: the summation order never varies
-    const float* src = a.part + static_cast<long long>(n) * a.bpi * g2;
-    for (int idx = tid; idx < parts * g2; idx += blockDim.x) {
-      const int k = idx % g2, part = idx / g2;
-      float acc = 0.f;
-      for (int b = part; b < a.bpi; b += parts) acc += src[static_cast<long long>(b) * g2 + k];
-      s_tot[part][k] = acc;
-    }
-    __syncthreads();
-    const float inv_cnt = 1.0f / (static_cast<float>(a.hw) * a.cpg);
-    for (int g = tid; g < a.groups; g += blockDim.x) {
-      float s = 0.f, q = 0.f;
-      for (int part = 0; part < parts; ++part) {
-        s += s_tot[part][2 * g];
-        q += s_tot[part][2 * g + 1];
-      }
-      const float dmean = s * inv_cnt;  // mean of x - K_g
-      float var = q * inv_cnt - dmean * dmean;
-      var = var < 0.f ? 0.f : var;
-      s_mean[g] += dmean;
-      s_rstd[g] = rsqrtf(var + a.eps);
-    }
-    __syncthreads();
-  }
   const int cv = tid % a.vecs;
   const int pl = tid / a.vecs;
   if (pl >= a.P) return;
@@ -222,6 +207,118 @@ __global__ void __launch_bounds__(kGnMaxThreads) gn_apply_kernel(GnArgs a) {
     o.w = C::pack(f[6], f[7]);
     *reinterpret_cast<uint4*>(static_cast<typename C::T*>(a.out) + pix * a.C + ch0) = o;
   }
+}
+
+// pass 2: image statistics from the slab partials (fixed order), then normalise + affine (+ SiLU)
+template <bool kBf16>
+__global__ void __launch_bounds__(kGnMaxThreads) gn_apply_kernel(GnArgs a) {
+  __shared__ float s_tot[4][128];
+  __shared__ float s_mean[64], s_rstd[64];
+  pdl_launch_dependents();
+  pdl_wait();
+  const int n = blockIdx.y;
+  const int tid = threadIdx.x;
+  const int g2 = a.groups * 2;
+  {
+    // K_g first (the same thread adds the shifted mean below): the load overlaps the partial sums
+    for (int g = tid; g < a.groups; g += blockDim.x) s_mean[g] = gn_shift<kBf16>(a, n, g);
+    const int parts = a.bpi >= 16 ? 4 : 1;  // a function of the shape only: the summation order never varies
+    const float* src = a.part + static_cast<long long>(n) * a.bpi * g2;
+    for (int idx = tid; idx < parts * g2; idx += blockDim.x) {
+      const int k = idx % g2, part = idx / g2;
+      float acc = 0.f;
+      for (int b = part; b < a.bpi; b += parts) acc += src[static_cast<long long>(b) * g2 + k];
+      s_tot[part][k] = acc;
+    }
+    __syncthreads();
+    const float inv_cnt = 1.0f / (static_cast<float>(a.hw) * a.cpg);
+    for (int g = tid; g < a.groups; g += blockDim.x) {
+      float s = 0.f, q = 0.f;
+      for (int part = 0; part < parts; ++part) {
+        s += s_tot[part][2 * g];
+        q += s_tot[part][2 * g + 1];
+      }
+      const float dmean = s * inv_cnt;  // mean of x - K_g
+      float var = q * inv_cnt - dmean * dmean;
+      var = var < 0.f ? 0.f : var;
+      s_mean[g] += dmean;
+      s_rstd[g] = rsqrtf(var + a.eps);
+    }
+    __syncthreads();
+  }
+  gn_normalise<kBf16>(a, n, s_mean, s_rstd);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Window mode (torch.nn.GroupNorm on [b, C, f, h, w]: one set of statistics per sample over all f frames).
+// Partial table: one record per (frame k, sample s), frame-major ([f][samples][rec]), so the tables of consecutive
+// frame slices concatenate into the table of the whole window. A record holds the K_g row (K_g, 0) of that frame's
+// image, then bpi slab rows of (sum, sumsq) of x - K_g; its length is padded to a multiple of 4 floats (16 bytes).
+// The reduction kernel adds, per sample and group, each frame's slabs in slab order, then moves the frame's sums to the
+// shift of frame 0 and adds them in frame order: the order depends on the frame and slab indices only, so a table
+// assembled from any frame-sharding gives bit-identical statistics.
+// ------------------------------------------------------------------------------------------------
+constexpr int kGnwReduceThreads = 256;
+constexpr int kGnwFrameChunk = 16;
+
+// one block per sample: stats[s][g] = (mean, rstd) over `table_frames` frames
+__global__ void __launch_bounds__(kGnwReduceThreads) gnw_reduce_kernel(GnArgs a, int table_frames, float* stats) {
+  __shared__ float s_tot[kGnwFrameChunk][128];
+  pdl_launch_dependents();
+  pdl_wait();
+  const int smp = blockIdx.x;
+  const int tid = threadIdx.x;
+  const int g2 = a.groups * 2;
+  const long long fstride = static_cast<long long>(a.samples) * a.rec;  // floats between frame k and k + 1
+  const float* base = a.part + static_cast<long long>(smp) * a.rec;
+  const float cnt = static_cast<float>(a.hw) * a.cpg;  // elements of one group in one frame
+  const float k0 = tid < a.groups ? base[2 * tid] : 0.f;
+  float S = 0.f, Q = 0.f;
+  for (int f0 = 0; f0 < table_frames; f0 += kGnwFrameChunk) {
+    const int nf = table_frames - f0 < kGnwFrameChunk ? table_frames - f0 : kGnwFrameChunk;
+    for (int idx = tid; idx < nf * g2; idx += blockDim.x) {
+      const int fi = idx / g2, k = idx - fi * g2;
+      const float* r = base + (f0 + fi) * fstride + g2 + k;
+      float acc = 0.f;
+#pragma unroll 8
+      for (int b = 0; b < a.bpi; ++b) acc += r[static_cast<long long>(b) * g2];
+      s_tot[fi][k] = acc;
+    }
+    __syncthreads();
+    if (tid < a.groups) {
+      for (int fi = 0; fi < nf; ++fi) {
+        const float d = base[(f0 + fi) * fstride + 2 * tid] - k0;  // K_g of this frame relative to frame 0's
+        const float sf = s_tot[fi][2 * tid], qf = s_tot[fi][2 * tid + 1];
+        // sum over the frame of (x - k0) and (x - k0)^2 from the sums of (x - K_f), (x - K_f)^2
+        S += sf + cnt * d;
+        Q += qf + d * (2.f * sf + cnt * d);
+      }
+    }
+    __syncthreads();
+  }
+  if (tid < a.groups) {
+    const float inv_cnt = 1.0f / (cnt * static_cast<float>(table_frames));
+    const float dmean = S * inv_cnt;
+    float var = Q * inv_cnt - dmean * dmean;
+    var = var < 0.f ? 0.f : var;
+    stats[(static_cast<long long>(smp) * a.groups + tid) * 2] = k0 + dmean;
+    stats[(static_cast<long long>(smp) * a.groups + tid) * 2 + 1] = rsqrtf(var + a.eps);
+  }
+}
+
+template <bool kBf16>
+__global__ void __launch_bounds__(kGnMaxThreads) gnw_apply_kernel(GnArgs a) {
+  __shared__ float s_mean[64], s_rstd[64];
+  pdl_launch_dependents();
+  pdl_wait();
+  const int n = blockIdx.y;
+  const float* st = a.stats + static_cast<long long>(n / a.frames) * a.groups * 2;
+  for (int g = threadIdx.x; g < a.groups; g += blockDim.x) {
+    s_mean[g] = st[2 * g];
+    s_rstd[g] = st[2 * g + 1];
+  }
+  __syncthreads();
+  gn_normalise<kBf16>(a, n, s_mean, s_rstd);
 }
 
 // launch geometry shared by mimo_groupnorm and mimo_groupnorm_workspace_bytes
@@ -518,6 +615,132 @@ extern "C" int mimo_groupnorm(const mimo_groupnorm_params* p, void* stream) {
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) return set_cuda_error("groupnorm launch", e);
   return MIMO_OK;
+}
+
+// ---- window mode ----
+static int gnw_check(const mimo_groupnorm_window_params* p, const char* who, int* Cout) {
+  static thread_local char msg[160];
+  auto fail = [&](const char* what) {
+    snprintf(msg, sizeof(msg), "%s: %s", who, what);
+    return set_error(MIMO_ERR_ARG, msg);
+  };
+  if (!p) return fail("null params");
+  if (p->samples <= 0 || p->frames <= 0 || p->hw <= 0 || p->groups <= 0 || p->groups > 64)
+    return fail("bad sizes (samples, frames, hw and groups must be > 0, groups <= 64)");
+  if (static_cast<long long>(p->samples) * p->frames > 65535) return fail("samples * frames must be <= 65535");
+  const int c1 = p->x1 ? p->c1 : 0;
+  const int C = p->c0 + c1;
+  if (p->c0 <= 0 || c1 < 0 || (p->c0 % 8) || (c1 % 8) || (C % p->groups) || (C / 8 > kGnMaxThreads))
+    return fail("channels must be multiples of 8, divisible by groups, <= 2560");
+  const int cpg = C / p->groups;
+  if (!(cpg >= 8 || cpg == 4)) return fail("channels per group must be 4 or >= 8");
+  if (p->dtype != MIMO_F16 && p->dtype != MIMO_BF16) return fail("dtype must be MIMO_F16 or MIMO_BF16");
+  *Cout = C;
+  return MIMO_OK;
+}
+
+// floats per (frame, sample) record: the K_g row and bpi slab rows of (sum, sumsq), padded to 16 bytes
+static long long gnw_rec_floats(const GnPlan& pl, int groups) {
+  return (2LL * groups * (pl.bpi + 1) + 3) / 4 * 4;
+}
+
+static GnArgs gnw_args(const mimo_groupnorm_window_params* p, int C, const GnPlan& pl) {
+  GnArgs a;
+  a.x0 = p->x0;
+  a.x1 = p->x1;
+  a.gamma = p->gamma;
+  a.beta = p->beta;
+  a.out = p->out;
+  a.part = p->table;
+  a.c0 = p->c0;
+  a.c1 = p->x1 ? p->c1 : 0;
+  a.C = C;
+  a.hw = p->hw;
+  a.groups = p->groups;
+  a.cpg = C / p->groups;
+  a.vecs = pl.vecs;
+  a.P = pl.P;
+  a.pix_per_block = pl.pix_per_block;
+  a.bpi = pl.bpi;
+  a.eps = p->eps;
+  a.silu = p->silu;
+  a.frames = p->frames;
+  a.samples = p->samples;
+  a.rec = gnw_rec_floats(pl, p->groups);
+  a.stats = p->stats;
+  return a;
+}
+
+static int64_t gnw_table_bytes(const mimo_groupnorm_window_params* p, int C, int frames) {
+  const GnPlan pl = gn_plan(p->samples * p->frames, p->hw, C);
+  return static_cast<int64_t>(frames) * p->samples * gnw_rec_floats(pl, p->groups) * static_cast<int64_t>(sizeof(float));
+}
+
+extern "C" int64_t mimo_groupnorm_window_table_bytes(const mimo_groupnorm_window_params* p) {
+  int C = 0;
+  if (int rc = gnw_check(p, "mimo_groupnorm_window_table_bytes", &C)) return rc;
+  return gnw_table_bytes(p, C, p->frames);
+}
+
+// the launches behind the three entry points: partials (pass 1), and/or reduce + normalise (pass 2)
+static int gnw_launch(const mimo_groupnorm_window_params* p, int C, bool partials, bool apply, int table_frames,
+                      void* stream) {
+  const GnPlan pl = gn_plan(p->samples * p->frames, p->hw, C);
+  const GnArgs a = gnw_args(p, C, pl);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const dim3 grid(pl.bpi, p->samples * p->frames);
+  const bool bf = p->dtype == MIMO_BF16;
+  cudaError_t e = cudaSuccess;
+  if (partials)
+    e = bf ? launch_k(gn_stats_kernel<true, true>, grid, dim3(pl.threads), 0, st, a)
+           : launch_k(gn_stats_kernel<false, true>, grid, dim3(pl.threads), 0, st, a);
+  if (apply && e == cudaSuccess) {
+    e = launch_k(gnw_reduce_kernel, dim3(p->samples), dim3(kGnwReduceThreads), 0, st, a, table_frames, p->stats);
+    if (e == cudaSuccess)
+      e = bf ? launch_k(gnw_apply_kernel<true>, grid, dim3(pl.threads), 0, st, a)
+             : launch_k(gnw_apply_kernel<false>, grid, dim3(pl.threads), 0, st, a);
+  }
+  if (e == cudaSuccess) e = cudaGetLastError();
+  if (e != cudaSuccess) return set_cuda_error("groupnorm_window launch", e);
+  return MIMO_OK;
+}
+
+extern "C" int mimo_groupnorm_window(const mimo_groupnorm_window_params* p, void* stream) {
+  const char* who = "mimo_groupnorm_window";
+  int C = 0;
+  if (int rc = gnw_check(p, who, &C)) return rc;
+  if (!p->x0 || !p->gamma || !p->beta || !p->out || !p->table || !p->stats)
+    return set_error(MIMO_ERR_ARG, "mimo_groupnorm_window: null pointer");
+  if (p->table_bytes < gnw_table_bytes(p, C, p->frames))
+    return set_error(MIMO_ERR_ARG, "mimo_groupnorm_window: partial table smaller than mimo_groupnorm_window_table_bytes");
+  if (int rc = ensure_device()) return rc;
+  return gnw_launch(p, C, true, true, p->frames, stream);
+}
+
+extern "C" int mimo_groupnorm_window_partials(const mimo_groupnorm_window_params* p, void* stream) {
+  const char* who = "mimo_groupnorm_window_partials";
+  int C = 0;
+  if (int rc = gnw_check(p, who, &C)) return rc;
+  if (!p->x0 || !p->table) return set_error(MIMO_ERR_ARG, "mimo_groupnorm_window_partials: null pointer");
+  if (p->table_bytes < gnw_table_bytes(p, C, p->frames))
+    return set_error(MIMO_ERR_ARG,
+                     "mimo_groupnorm_window_partials: partial table smaller than mimo_groupnorm_window_table_bytes");
+  if (int rc = ensure_device()) return rc;
+  return gnw_launch(p, C, true, false, 0, stream);
+}
+
+extern "C" int mimo_groupnorm_window_apply(const mimo_groupnorm_window_params* p, void* stream) {
+  const char* who = "mimo_groupnorm_window_apply";
+  int C = 0;
+  if (int rc = gnw_check(p, who, &C)) return rc;
+  if (p->table_frames < p->frames)
+    return set_error(MIMO_ERR_ARG, "mimo_groupnorm_window_apply: table_frames must be >= frames (the whole window)");
+  if (!p->x0 || !p->gamma || !p->beta || !p->out || !p->table || !p->stats)
+    return set_error(MIMO_ERR_ARG, "mimo_groupnorm_window_apply: null pointer");
+  if (p->table_bytes < gnw_table_bytes(p, C, p->table_frames))
+    return set_error(MIMO_ERR_ARG, "mimo_groupnorm_window_apply: partial table smaller than table_frames records");
+  if (int rc = ensure_device()) return rc;
+  return gnw_launch(p, C, false, true, p->table_frames, stream);
 }
 
 extern "C" int mimo_layernorm(const void* x, const void* gamma, const void* beta, void* out, int64_t rows,

@@ -18,7 +18,7 @@ Algebraic folds (identical results up to rounding order; see DESIGN.md):
 from __future__ import annotations
 
 import math
-from dataclasses import dataclass
+from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
@@ -42,6 +42,10 @@ class UNetSpec:
     out_channels: int = 4
     motion: bool = True
     out_head: bool = True
+    # ResnetBlock3D norm1 / norm2 and conv_norm_out: per frame (InflatedGroupNorm, resnet.py:20-28) or, when False, one
+    # torch.nn.GroupNorm over all frames of the window (resnet.py:155-163, 185-192; unet_3d_edit_bkfill.py:236-247).
+    # The packed weights do not depend on it, so it stays out of the repr that keys the weight cache.
+    inflated_groupnorm: bool = field(default=True, repr=False)
 
 
 def _dev(sd: SD, key: str, device, dtype) -> torch.Tensor:
@@ -257,15 +261,42 @@ class UNetEngine:
     def _time_embed(self, timesteps: torch.Tensor) -> torch.Tensor:
         return self._time_embed_from(self._sinusoid(timesteps))
 
+    def _norm_silu(self, x0, gb, n, hw, rows_per_branch, window: bool, slot: str, x1=None):
+        """SiLU(GroupNorm) of a ResnetBlock3D or of conv_norm_out (eps = norm_eps). Per frame, or with `window` over
+        all frames of each CFG branch (rows_per_branch = frames * hw). Frame-sharded (self.xchg, G GPUs): every member
+        writes the partial table of its frames into its peer buffer `slot`, the group all-gathers the tables (bytes
+        moved as they are) and every member normalises its frames from the whole window's table."""
+        g, eps = self.spec.norm_num_groups, self.spec.norm_eps
+        if not window:
+            return ops.groupnorm(x0, *gb, n, hw, groups=g, eps=eps, silu=True, x1=x1)
+        f = rows_per_branch // hw
+        b = n // f
+        xg = self.xchg
+        if xg is None or xg.G == 1:
+            return ops.groupnorm_window(x0, *gb, b, f, hw, groups=g, eps=eps, silu=True, x1=x1)
+        c = x0.shape[1] + (x1.shape[1] if x1 is not None else 0)
+        need = ops.groupnorm_window_table_bytes(b, f, hw, c, g)
+        if slot not in xg.bufs or xg.bufs[slot].nbytes < need:
+            raise L.MimoError(f"frame-sharded window GroupNorm needs a peer buffer '{slot}' of {need} bytes")
+        mine = xg.bufs[slot].bytes[:need].view(torch.float32)
+        ops.groupnorm_window_partials(x0, b, f, hw, groups=g, x1=x1, table=mine)
+        table = torch.empty((xg.G * need // 4,), dtype=torch.float32, device=x0.device)
+        xg.pull(2, slot, table.view(torch.float16).view(-1, 8), 1, 1, need // 16, 8)  # fp32 bytes as 16-bit pairs
+        return ops.groupnorm_window_apply(x0, *gb, table, b, f, f * xg.G, hw, groups=g, eps=eps, silu=True, x1=x1)
+
+    _window_gn = False  # whether the forward being recorded runs the ResBlocks' GroupNorms over the window (_forward_impl)
+
     def _resnet(self, p, x0, x1, tembs, n, h, w, rows_per_branch):
         r = self.w[p]
-        g, eps = self.spec.norm_num_groups, self.spec.norm_eps
         hw = h * w
-        t = ops.groupnorm(x0, *r["n1"], n, hw, groups=g, eps=eps, silu=True, x1=x1)
+        window_gn = self._window_gn
+        # window mode, frame-sharded: norm1 and norm2 gather through two peer buffers used alternately, so a member only
+        # rewrites one after the exchange in between (csrc/exchange.cu); the output norm has a third
+        t = self._norm_silu(x0, r["n1"], n, hw, rows_per_branch, window_gn, "N0", x1=x1)
         off, cout = self.temb_off[p]
         t = ops.conv3x3(t, r["c1"][0], n, h, w, bias=r["c1"][1], rowvec=tembs[:, off:off + cout],
                         rows_per_group=rows_per_branch)
-        t = ops.groupnorm(t, *r["n2"], n, hw, groups=g, eps=eps, silu=True)
+        t = self._norm_silu(t, r["n2"], n, hw, rows_per_branch, window_gn, "N1")
         if r["sc"] is not None:
             res = ops.gemm(x0, r["sc"][0], a1=x1, bias=r["sc"][1])
         else:
@@ -509,9 +540,12 @@ class UNetEngine:
         wci, bci = self.w["conv_in"]
         x = ops.conv3x3(x_in, wci, b * f, h, w, bias=bci, residual=pose_nhwc)
         xf = lambda p, xx, n, hw, rpb: self._xf_read(p, xx, n, hw, rpb, st)
-        x, h2, w2 = self._body(x, tembs, b, f, h, w, xf)
-        x = ops.groupnorm(x, *self.w["norm_out"], b * f, h * w, groups=self.spec.norm_num_groups,
-                          eps=self.spec.norm_eps, silu=True)
+        self._window_gn = window = not self.spec.inflated_groupnorm
+        try:
+            x, h2, w2 = self._body(x, tembs, b, f, h, w, xf)
+        finally:
+            self._window_gn = False
+        x = self._norm_silu(x, self.w["norm_out"], b * f, h * w, f * h * w, window, "N2")
         wco, bco = self.w["conv_out"]
         y = ops.conv3x3(x, wco, b * f, h, w, bias=bco)
         return ops.nhwc_to_ncfhw(y, b, self.spec.out_channels, f, h, w)

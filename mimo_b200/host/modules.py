@@ -261,9 +261,14 @@ class UNet3DConditionModel(_UNetBase):
         if unsupported:
             raise NotImplementedError("mimo_b200.UNet3DConditionModel: " + "; ".join(unsupported))
         self._motion_max_len = mk.get("temporal_position_encoding_max_len", 32)
+        # False (the reference's default): ResnetBlock3D norm1 / norm2 and conv_norm_out are torch.nn.GroupNorm over all
+        # frames of a window (resnet.py:155-163, 185-192; unet_3d_edit_bkfill.py:236-247); True: per frame
+        self.use_inflated_groupnorm = bool(use_inflated_groupnorm)
         self._init_unet(block_out_channels, layers_per_block, cross_attention_dim, attention_head_dim, norm_num_groups,
                         norm_eps, 8, out_channels,  # in_channels is forced to 8 (unet_3d_edit_bkfill.py:88)
-                        dict(sample_size=sample_size), motion_max_len=self._motion_max_len)
+                        dict(sample_size=sample_size, use_inflated_groupnorm=self.use_inflated_groupnorm),
+                        motion_max_len=self._motion_max_len)
+        self._spec.inflated_groupnorm = self.use_inflated_groupnorm
 
     @classmethod
     def from_pretrained_2d(cls, pretrained_model_path, motion_module_path, subfolder=None,

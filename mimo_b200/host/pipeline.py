@@ -212,7 +212,12 @@ class Pose2VideoPipeline:
             c0 = self.denoising_unet.config.block_out_channels[0]
             tok = nb * fl * h * w * c0 * esz  # the widest token tensor of a forward: the first level's
             kw = dict(timeout_ms=getattr(self, "_xchg_timeout_ms", 0))
-            self._xchg_frame = (Exchange.create(plan.frame_group(), rank, {"A": tok, "B": tok}, self.device, group, **kw)
+            sizes = {"A": tok, "B": tok}
+            if not getattr(self.denoising_unet, "use_inflated_groupnorm", True):
+                # window GroupNorm: the per-frame partial tables of ResnetBlock3D norm1 / norm2 / conv_norm_out
+                t = self._window_table_bytes(nb, fl, h, w)
+                sizes.update(N0=t, N1=t, N2=t)
+            self._xchg_frame = (Exchange.create(plan.frame_group(), rank, sizes, self.device, group, **kw)
                                 if plan.frame_ways > 1 else None)
             # two gather sources used alternately: a source may only be rewritten once every peer has announced the NEXT
             # exchange (= finished pulling this one), i.e. after one exchange in between (csrc/exchange.cu)
@@ -220,6 +225,15 @@ class Pose2VideoPipeline:
             self._xchg_world = Exchange.create(list(range(world)), rank, {"S0": sz, "S1": sz}, self.device, group, **kw)
             self._xchg_key = key
         return self._xchg_frame, self._xchg_world
+
+    def _window_table_bytes(self, nb: int, fl: int, h: int, w: int) -> int:
+        """The largest window-GroupNorm partial table of one member's fl frames: every ResnetBlock3D input / output
+        width (up-block inputs include the skip) at every level of an h x w latent."""
+        cfg = self.denoising_unet.config
+        ch = list(cfg.block_out_channels)
+        widths = set(ch) | {a + b for a in ch for b in ch}
+        return max(ops.groupnorm_window_table_bytes(nb, fl, lh * lw, c, cfg.norm_num_groups)
+                   for lh, lw in E.latent_levels(h, w, len(ch)) for c in widths if c % cfg.norm_num_groups == 0)
 
     # ------------------------------------------------------------------------------------------------
     def to(self, device=None, dtype=None):

@@ -73,6 +73,22 @@ class GroupNormParams(C.Structure):
     ]
 
 
+class GroupNormWindowParams(C.Structure):
+    _fields_ = [
+        ("x0", C.c_void_p), ("c0", C.c_int32),
+        ("x1", C.c_void_p), ("c1", C.c_int32),
+        ("gamma", C.c_void_p), ("beta", C.c_void_p),
+        ("out", C.c_void_p),
+        ("table", C.c_void_p), ("table_bytes", C.c_int64),
+        ("stats", C.c_void_p),
+        ("samples", C.c_int32), ("frames", C.c_int32), ("table_frames", C.c_int32), ("hw", C.c_int32),
+        ("groups", C.c_int32),
+        ("eps", C.c_float),
+        ("silu", C.c_int32),
+        ("dtype", C.c_int32),
+    ]
+
+
 class AttnParams(C.Structure):
     _fields_ = [
         ("q", C.c_void_p), ("k", C.c_void_p), ("v", C.c_void_p), ("ld_qkv", C.c_int64),
@@ -137,6 +153,10 @@ SYMBOLS = {
     "mimo_im2col3x3": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I64, _I32, _VP]),
     "mimo_groupnorm": (C.c_int, [C.POINTER(GroupNormParams), _VP]),
     "mimo_groupnorm_workspace_bytes": (C.c_int64, [C.POINTER(GroupNormParams)]),
+    "mimo_groupnorm_window": (C.c_int, [C.POINTER(GroupNormWindowParams), _VP]),
+    "mimo_groupnorm_window_partials": (C.c_int, [C.POINTER(GroupNormWindowParams), _VP]),
+    "mimo_groupnorm_window_apply": (C.c_int, [C.POINTER(GroupNormWindowParams), _VP]),
+    "mimo_groupnorm_window_table_bytes": (C.c_int64, [C.POINTER(GroupNormWindowParams)]),
     "mimo_layernorm": (C.c_int, [_VP, _VP, _VP, _VP, _I64, _I32, _F, _VP, _I64, _I32, _I32, _I32, _VP]),
     "mimo_attn_spatial": (C.c_int, [C.POINTER(AttnParams), _VP]),
     "mimo_attn_temporal": (C.c_int, [C.POINTER(AttnTemporalParams), _VP]),
@@ -182,7 +202,7 @@ def load() -> C.CDLL:
         fn.restype = res
         fn.argtypes = args
     for which, st in enumerate((Epilogue, GemmParams, Conv3x3Params, GroupNormParams, AttnParams, AttnTemporalParams,
-                             ExchangeParams, CfgMultistepParams)):
+                             ExchangeParams, CfgMultistepParams, GroupNormWindowParams)):
         if lib.mimo_abi_sizeof(which) != C.sizeof(st):
             raise MimoError(f"ABI mismatch: {st.__name__} is {C.sizeof(st)} bytes in lib.py but "
                             f"{lib.mimo_abi_sizeof(which)} in {LIB_PATH.name}; rebuild the library")

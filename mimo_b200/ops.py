@@ -221,6 +221,86 @@ def groupnorm(x0: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, n: int,
     return out
 
 
+def _gnw_params(x0, samples, frames, hw, groups, *, x1=None, gamma=None, beta=None, out=None, table=None, stats=None,
+                table_frames=0, eps=1e-5, silu=False, dtype=None) -> L.GroupNormWindowParams:
+    p = L.GroupNormWindowParams()
+    p.x0, p.c0 = _ptr(x0), x0.shape[1]
+    p.x1, p.c1 = _ptr(x1), (x1.shape[1] if x1 is not None else 0)
+    p.gamma, p.beta, p.out, p.stats = _ptr(gamma), _ptr(beta), _ptr(out), _ptr(stats)
+    p.table, p.table_bytes = _ptr(table), (table.numel() * table.element_size() if table is not None else 0)
+    p.samples, p.frames, p.table_frames, p.hw, p.groups = int(samples), int(frames), int(table_frames), int(hw), int(groups)
+    p.eps, p.silu, p.dtype = float(eps), int(bool(silu)), _dt(x0) if dtype is None else dtype
+    return p
+
+
+def groupnorm_window_table_bytes(samples: int, frames: int, hw: int, channels: int, groups: int = 32) -> int:
+    """Bytes of the window-mode partial table of `frames` frames of `samples` samples (no GPU needed)."""
+    p = L.GroupNormWindowParams(c0=int(channels), samples=int(samples), frames=int(frames), hw=int(hw),
+                                groups=int(groups), dtype=L.F16)
+    need = L.load().mimo_groupnorm_window_table_bytes(C.byref(p))
+    if need < 0:
+        L.check(int(need), "mimo_groupnorm_window_table_bytes")
+    return int(need)
+
+
+def _gnw_table(table: Optional[torch.Tensor], need: int, device) -> torch.Tensor:
+    if table is None:
+        return torch.empty((need // 4,), dtype=torch.float32, device=device)
+    assert table.dtype == torch.float32 and table.is_contiguous() and table.numel() * 4 >= need
+    return table
+
+
+def groupnorm_window(x0: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, samples: int, frames: int, hw: int, *,
+                     groups=32, eps=1e-5, silu=False, x1: Optional[torch.Tensor] = None,
+                     out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """torch.nn.GroupNorm(+SiLU) over [samples, C, frames, h, w] on channels-last x0 [samples*frames*hw, c0] (+ x1):
+    one set of statistics per sample and group over all `frames` frames."""
+    c = x0.shape[1] + (x1.shape[1] if x1 is not None else 0)
+    assert x0.is_contiguous() and (x1 is None or x1.is_contiguous()) and x0.shape[0] == samples * frames * hw
+    if out is None:
+        out = torch.empty((samples * frames * hw, c), dtype=x0.dtype, device=x0.device)
+    assert out.is_contiguous()
+    table = _gnw_table(None, groupnorm_window_table_bytes(samples, frames, hw, c, groups), x0.device)
+    stats = torch.empty((samples * groups * 2,), dtype=torch.float32, device=x0.device)
+    p = _gnw_params(x0, samples, frames, hw, groups, x1=x1, gamma=gamma, beta=beta, out=out, table=table, stats=stats,
+                    table_frames=frames, eps=eps, silu=silu)
+    with _Call("groupnorm", 3, 0.0, 2.0 * 2 * out.numel()):
+        L.check(L.load().mimo_groupnorm_window(C.byref(p), _stream()), "mimo_groupnorm_window")
+    return out
+
+
+def groupnorm_window_partials(x0: torch.Tensor, samples: int, frames: int, hw: int, *, groups=32,
+                              x1: Optional[torch.Tensor] = None, table: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The window-mode partial table of x0's `frames` frames (fp32, frame-major: tables of consecutive frame slices
+    concatenate into the whole window's). `table`: an fp32 buffer to write it to (e.g. a peer-memory source)."""
+    c = x0.shape[1] + (x1.shape[1] if x1 is not None else 0)
+    assert x0.is_contiguous() and (x1 is None or x1.is_contiguous()) and x0.shape[0] == samples * frames * hw
+    table = _gnw_table(table, groupnorm_window_table_bytes(samples, frames, hw, c, groups), x0.device)
+    p = _gnw_params(x0, samples, frames, hw, groups, x1=x1, table=table)
+    with _Call("groupnorm", 1, 0.0, 2.0 * x0.shape[0] * c):
+        L.check(L.load().mimo_groupnorm_window_partials(C.byref(p), _stream()), "mimo_groupnorm_window_partials")
+    return table
+
+
+def groupnorm_window_apply(x0: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, table: torch.Tensor, samples: int,
+                           frames: int, table_frames: int, hw: int, *, groups=32, eps=1e-5, silu=False,
+                           x1: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Normalise x0's `frames` frames (+ affine, SiLU) with the statistics of a partial table that covers all
+    `table_frames` frames of the window."""
+    c = x0.shape[1] + (x1.shape[1] if x1 is not None else 0)
+    assert x0.is_contiguous() and (x1 is None or x1.is_contiguous()) and x0.shape[0] == samples * frames * hw
+    if out is None:
+        out = torch.empty((samples * frames * hw, c), dtype=x0.dtype, device=x0.device)
+    assert out.is_contiguous()
+    table = _gnw_table(table, groupnorm_window_table_bytes(samples, table_frames, hw, c, groups), x0.device)
+    stats = torch.empty((samples * groups * 2,), dtype=torch.float32, device=x0.device)
+    p = _gnw_params(x0, samples, frames, hw, groups, x1=x1, gamma=gamma, beta=beta, out=out, table=table, stats=stats,
+                    table_frames=table_frames, eps=eps, silu=silu)
+    with _Call("groupnorm", 2, 0.0, 2.0 * 2 * out.numel()):
+        L.check(L.load().mimo_groupnorm_window_apply(C.byref(p), _stream()), "mimo_groupnorm_window_apply")
+    return out
+
+
 def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, *, eps=1e-5, pe: Optional[torch.Tensor] = None,
               rows_per_frame=1, frames=1, pe_frame_offset=0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     assert x.is_contiguous() and x.dim() == 2

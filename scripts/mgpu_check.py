@@ -25,6 +25,8 @@ def main():
     ap.add_argument("--out", default=None)
     ap.add_argument("--full-width", action="store_true", help="full SD1.5 width instead of the reduced test width")
     ap.add_argument("--frames", type=int, nargs="*", default=None, help="only the cases with these frame counts")
+    ap.add_argument("--window-groupnorm", action="store_true",
+                    help="denoising UNet built with use_inflated_groupnorm=False (ResBlock GroupNorms over the window)")
     args = ap.parse_args()
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     torch.cuda.set_device(local)
@@ -55,7 +57,8 @@ def main():
     seed = 700
     mk = dict(num_attention_heads=8, num_transformer_block=1, attention_block_types=["Temporal_Self", "Temporal_Self"],
               temporal_position_encoding=True, temporal_position_encoding_max_len=32, temporal_attention_dim_div=1)
-    den = M.UNet3DConditionModel(block_out_channels=widths, cross_attention_dim=768, use_inflated_groupnorm=True,
+    den = M.UNet3DConditionModel(block_out_channels=widths, cross_attention_dim=768,
+                                 use_inflated_groupnorm=not args.window_groupnorm,
                                  use_motion_module=True, motion_module_mid_block=True, motion_module_type="Vanilla",
                                  motion_module_kwargs=mk)
     ref = M.UNet2DConditionModel(block_out_channels=widths, cross_attention_dim=768)
