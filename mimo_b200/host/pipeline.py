@@ -4,11 +4,13 @@
 What stays as in the reference: PIL pre-processing semantics, CLIP through the HF module the caller passes, the CPU
 generator noise (prepare_latents :149-183), context windows (:492-510), CFG (:545-549) and scheduler (:551-553) maths.
 What changes is where the arithmetic runs: reference_unet / pose_guider / denoising_unet / VAE are engine objects
-behind the C ABI; the CFG + DDIM update (also with eta > 0) is one fused kernel, the CFG + DPM-Solver++ / Euler /
-Euler-ancestral update another (host/scheduler.py: engine_scheduler), latent frame interpolation a third; the
-frames are decoded in batched VAE passes (one pass up to DECODE_PIXELS_PER_PASS output pixels).
+behind the C ABI; each step's CFG + scheduler update is one fused kernel that the scheduler runs itself
+(host/scheduler.py: fused_step), latent frame interpolation another; the frames are decoded in batched VAE passes (one
+pass up to DECODE_PIXELS_PER_PASS output pixels).
 
-__call__ = preprocess() [host: PIL -> pinned tensors]  ->  H2D  ->  sample_tensors() [device]  ->  D2H.
+__call__ = preprocess() [host: PIL -> pinned tensors]  ->  H2D  ->  sample_tensors() [device]  ->  D2H, and
+sample_tensors() = _check_sampling -> CLIP -> _encode_vae -> _pose_features -> _shard_plan + _reference_pass
+-> _denoise -> [interpolation] -> _decode, each phase timed by CUDA events (timings).
 """
 from __future__ import annotations
 
@@ -18,12 +20,15 @@ from typing import Callable, Dict, List, Optional, Union
 import numpy as np
 import PIL.Image
 import torch
+import torch.distributed as dist
 
 from .. import engine as E
 from .. import ops
 from ..lib import MimoError
 from .context import get_context_scheduler
 from .modules import ReferenceAttentionControl
+from .scheduler import engine_scheduler
+from .shard import Exchange, ShardPlan, gather_layout
 
 
 @dataclass
@@ -160,6 +165,13 @@ def _randn_tensor(shape, generator, device: torch.device, dtype) -> torch.Tensor
     return torch.randn(shape, generator=generator, device=gdev, dtype=dtype).to(device)
 
 
+def _all_gather_rows(local: torch.Tensor, world: int, group) -> torch.Tensor:
+    """[n, ...] of every rank -> [world * n, ...] in rank order: one all_gather_into_tensor."""
+    out = torch.empty((world * local.shape[0],) + tuple(local.shape[1:]), dtype=local.dtype, device=local.device)
+    dist.all_gather_into_tensor(out, local.contiguous(), group=group)
+    return out
+
+
 class Pose2VideoPipeline:
     _optional_components: list = []
 
@@ -176,6 +188,9 @@ class Pose2VideoPipeline:
         self.last_latents: Optional[torch.Tensor] = None
         self.io_bytes = {"h2d": 0, "d2h": 0}
         self._shard = (0, 1, None)  # (rank, world, process group): see enable_sharding()
+        self.force_plan = None  # (cfg_ways, win_ways, frame_ways) instead of ShardPlan.make's: tests exercise every axis
+        self._xchg_frame = self._xchg_world = self._xchg_key = None  # see _exchanges()
+        self._xchg_retired, self._xchg_timeout_ms = [], 0
 
     def enable_sharding(self, rank: int, world: int, group=None, exchange_timeout_ms: int = 0):
         """Partition every clip over `world` GPUs (one process per GPU, torch.distributed already initialised):
@@ -193,25 +208,24 @@ class Pose2VideoPipeline:
         """Collective (every rank calls it): unmap and free the peer buffers of exchanges that were replaced because the
         clip geometry or the partitioning changed. The exchanges in use stay."""
         _, _, group = self._shard
-        for x in self.__dict__.pop("_xchg_retired", []):
+        retired, self._xchg_retired = self._xchg_retired, []
+        for x in retired:
             x.destroy(group)
 
     def _exchanges(self, plan, nb: int, n_my_windows: int, fl: int, h: int, w: int, dtype):
         """(frame-group exchange or None, world exchange): peer buffers sized for this geometry; collective."""
-        from .shard import Exchange
         rank, world, group = self._shard
         key = (plan, nb, n_my_windows, fl, h, w, dtype)
-        if getattr(self, "_xchg_key", None) != key:
+        if self._xchg_key != key:
             # captured forwards hold the old buffers' addresses: drop the graphs; the old exchanges are retired, not
             # freed (freeing peer-mapped memory is a collective: release_exchanges() does it when the caller wants to)
             self.denoising_unet.engine()._graphs.clear()
-            retired = self.__dict__.setdefault("_xchg_retired", [])
-            retired += [x for x in (getattr(self, "_xchg_frame", None), getattr(self, "_xchg_world", None)) if x is not None]
+            self._xchg_retired += [x for x in (self._xchg_frame, self._xchg_world) if x is not None]
             self._xchg_frame = self._xchg_world = None
             esz = torch.empty((), dtype=dtype).element_size()
             c0 = self.denoising_unet.config.block_out_channels[0]
             tok = nb * fl * h * w * c0 * esz  # the widest token tensor of a forward: the first level's
-            kw = dict(timeout_ms=getattr(self, "_xchg_timeout_ms", 0))
+            kw = dict(timeout_ms=self._xchg_timeout_ms)
             sizes = {"A": tok, "B": tok}
             if not getattr(self.denoising_unet, "use_inflated_groupnorm", True):
                 # window GroupNorm: the per-frame partial tables of ResnetBlock3D norm1 / norm2 / conv_norm_out
@@ -350,23 +364,15 @@ class Pose2VideoPipeline:
                                len(self.denoising_unet.config.block_out_channels))
 
     # ------------------------------------------------------------------------------------------------
-    @staticmethod
-    def _step_draws(sched, eta: float) -> bool:
-        """Whether every step of `sched` consumes one randn_tensor(model_output.shape) draw: DDIM with eta > 0
-        (DDIMScheduler.step [3P]) and Euler-ancestral; eta reaches DDIM only (prepare_extra_step_kwargs, :128-147)."""
-        from .scheduler import DDIMScheduler
-        return eta > 0 if isinstance(sched, DDIMScheduler) else sched.draws_noise
-
     def _draw_noise(self, width, height, video_length, dtype, generator, num_inference_steps: int, eta: float,
-                    pinned: bool, sched=None):
+                    pinned: bool, sched):
         """The clip's random draws in the reference's order: the initial latents (prepare_latents, scaled by `sched`'s
-        init_noise_sigma), then, for schedulers whose steps consume a draw (_step_draws) and with a generator, one
+        init_noise_sigma), then, for schedulers whose steps consume a draw (step_draws) and with a generator, one
         randn_tensor(model_output.shape) per step (also at the last step), stacked in one (pinned) tensor
         [steps, 1, 4, F, h, w]. Without a generator the step noise is drawn on the device inside the loop, as
         randn_tensor does."""
-        sched = sched if sched is not None else self.scheduler
         latents = self.prepare_latents(1, 4, width, height, video_length, dtype, "cpu", generator, scheduler=sched)
-        if not (self._step_draws(sched, eta) and generator is not None and num_inference_steps > 0):
+        if not (sched.step_draws(eta) and generator is not None and num_inference_steps > 0):
             return latents, None
         shape = tuple(latents.shape)
         noise = torch.empty((num_inference_steps,) + shape, dtype=dtype, pin_memory=pinned)
@@ -379,7 +385,6 @@ class Pose2VideoPipeline:
         """Host side of __call__: PIL -> pinned CPU tensors (what the reference does at pipeline :379-381, :409-418,
         :424-426, :435-437, :446-453 before anything touches the device). With a generator, the per-step noise of DDIM
         with eta > 0 or of Euler-ancestral is drawn here too, right after the initial latents, as "step_noise"."""
-        from .scheduler import engine_scheduler
         sched = engine_scheduler(self.scheduler)
         if num_inference_steps > 0:
             sched.set_timesteps(num_inference_steps, device="cpu")  # init_noise_sigma may depend on the table
@@ -428,126 +433,140 @@ class Pose2VideoPipeline:
                        context_schedule="uniform", context_frames=24, context_stride=1, context_overlap=4,
                        callback=None, callback_steps=1, decode: bool = True, eta: float = 0.0,
                        interpolation_factor: int = 1) -> Dict[str, torch.Tensor]:
-        """Device side: everything in `inp` already lives in HBM; returns device tensors. eta > 0: stochastic DDIM with
-        inp["step_noise"] [steps, 1, 4, F, h, w] (preprocess draws it from the generator), or, without it, noise drawn
-        on the device at every step. interpolation_factor k >= 2: the registered interpolation method inserts k-1
-        frames between neighbours before the decode; out["latents"] stays the denoised clip.
-        The scheduler is engine_scheduler(self.scheduler): DDIM runs mimo_cfg_ddim_step(_noise), DPM-Solver++, Euler and
-        Euler-ancestral one mimo_cfg_multistep per step (Euler-ancestral with inp["step_noise"] or device draws, as
-        eta > 0 does)."""
-        from .scheduler import DDIMScheduler, engine_scheduler
-        device = self.device
-        dtype = self.denoising_unet.dtype
-        do_cfg = guidance_scale > 1.0
+        """Device side: everything in `inp` already lives in HBM; returns device tensors. The scheduler is
+        engine_scheduler(self.scheduler); each step is one fused kernel: mimo_cfg_ddim_step(_noise) for DDIM,
+        mimo_cfg_multistep for DPM-Solver++, Euler and Euler-ancestral. The per-step noise of eta > 0 (stochastic DDIM)
+        and of Euler-ancestral is inp["step_noise"] [steps, 1, 4, F, h, w] (preprocess draws it from the generator) or,
+        without it, drawn on the device at every step. interpolation_factor k >= 2: the registered interpolation method
+        inserts k-1 frames between neighbours before the decode; out["latents"] stays the denoised clip."""
+        sched, interp, step_noise = self._check_sampling(inp, num_inference_steps, eta, interpolation_factor)
+        dtype, do_cfg = self.denoising_unet.dtype, guidance_scale > 1.0
+        marks = []
+
+        def mark(name):
+            marks.append((name, torch.cuda.Event(enable_timing=True)))
+            marks[-1][1].record()
+
+        mark("start")
+        sched.set_timesteps(num_inference_steps, device="cpu")
+        timesteps = [t.item() for t in sched.timesteps]  # DDIM / DPM-Solver++: int; Euler: fp32 values
+        ehs = self._clip().image_embeds(inp["clip_pixels"]).to(dtype).unsqueeze(1)  # :378-385
+        ehs = torch.cat([torch.zeros_like(ehs), ehs], dim=0) if do_cfg else ehs
+        mark("clip")
+        latents = inp["latents"].to(dtype).clone()
+        F_, h, w = latents.shape[2:]
+        ref_latents, vid_bk, pose_px = self._encode_vae(inp, dtype, h, w)
+        mark("vae_encode")
+        pose_fea = self._pose_features(pose_px, F_, h, w)
+        mark("pose_guider")
+        windows = list(get_context_scheduler(context_schedule)(0, num_inference_steps, F_, context_frames,
+                                                               context_stride, context_overlap))
+        plan = self._shard_plan(windows, do_cfg, h, w)
+        branches = plan.branches(do_cfg) if plan else tuple(range(2 if do_cfg else 1))
+        reader, writer = self._reference_pass(ref_latents, ehs, do_cfg, branches, dtype)
+        mark("reference_unet")
+        self._denoise(sched, timesteps, latents, windows, plan, branches, pose_fea, vid_bk, guidance_scale, eta,
+                      step_noise, callback, callback_steps)
+        mark("denoise")
+        reader.clear()
+        writer.clear()
+        out = {"latents": latents}
+        if decode:
+            vid_lat = latents
+            if interp is not None:  # pipeline :566-567: the frames to decode, (F - 1) * k + 1 of them
+                vid_lat = ops.interpolate_frames(latents, interpolation_factor, interp)
+                mark("interpolate")
+            out["videos"] = self._decode(vid_lat)
+            mark("vae_decode")
+        self._marks = marks
+        self.last_latents = latents
+        return out
+
+    def _check_sampling(self, inp, num_inference_steps: int, eta: float, interpolation_factor: int):
+        """The refusals, in this order, before any work -> (scheduler, interpolation method, step noise or None)."""
         if eta < 0:
             raise ValueError(f"eta={eta}: DDIM's eta is >= 0 (0 deterministic, 1 DDPM-like)")
         interp = self._interpolation_method(interpolation_factor, inp["latents"].shape[2])
         sched = engine_scheduler(self.scheduler)
-        ddim = isinstance(sched, DDIMScheduler)
-        draws = self._step_draws(sched, eta)
-        step_noise = inp.get("step_noise") if draws else None
+        step_noise = inp.get("step_noise") if sched.step_draws(eta) else None
         if step_noise is not None and (step_noise.shape[0] < num_inference_steps
                                        or tuple(step_noise.shape[1:]) != tuple(inp["latents"].shape)):
             raise ValueError(f"step_noise {tuple(step_noise.shape)} does not hold {num_inference_steps} draws of "
                              f"{tuple(inp['latents'].shape)}")
-        ev = lambda: torch.cuda.Event(enable_timing=True)
-        marks = [("start", ev())]
-        marks[0][1].record()
+        return sched, interp, step_noise
 
-        def mark(name):
-            e = ev()
-            e.record()
-            marks.append((name, e))
-
-        sched.set_timesteps(num_inference_steps, device="cpu")
-        timesteps = [t.item() for t in sched.timesteps]  # DDIM / DPM-Solver++: int; Euler: fp32 values
-
-        emb = self._clip().image_embeds(inp["clip_pixels"]).to(dtype)  # :378-385
-        ehs = emb.unsqueeze(1)
-        if do_cfg:
-            ehs = torch.cat([torch.zeros_like(ehs), ehs], dim=0)
-        mark("clip")
-
-        latents = inp["latents"].to(dtype).clone()
-        F_, h, w = latents.shape[2], latents.shape[3], latents.shape[4]
+    def _encode_vae(self, inp, dtype, h: int, w: int):
+        """-> (reference latents, background latents [1, 4, F, h, w], pose pixels [1, 3, F, H, W]): every image goes
+        from bytes to normalised pixels on the device here (pipeline :424-426, :435-437, :446-453)."""
         enc, _ = self._vae()
-        # bytes -> normalised pixels on the device (pipeline :424-426, :435-437, :446-453)
         ref_px = uint8_to_tensor(inp["ref_u8"], True).to(dtype)
         bk_px = uint8_to_tensor(inp["bk_unique_u8"], True).to(dtype)
-        pose_px = uint8_to_tensor(inp["pose_u8"], False).permute(1, 0, 2, 3).unsqueeze(0).to(dtype)  # [1, 3, F, H, W]
+        pose_px = uint8_to_tensor(inp["pose_u8"], False).permute(1, 0, 2, 3).unsqueeze(0).to(dtype)
         rank, world, group = self._shard
         n_bk = bk_px.shape[0]
-        if not (world > 1 and n_bk >= world) and n_bk <= 4:
+        if world > 1 and n_bk >= world:
+            # edit mode: one distinct background per frame (run_edit.py:232-238) - every GPU encodes its share, one
+            # all-gather per clip (per-image arithmetic: identical to encoding them all here)
+            ref_latents = enc.encode_mean(ref_px) * 0.18215  # :424-431
+            per = -(-n_bk // world)
+            lo, hi = min(rank * per, n_bk), min((rank + 1) * per, n_bk)
+            mine = torch.zeros((per, 4, h, w), device=self.device, dtype=dtype)
+            if hi > lo:
+                mine[:hi - lo] = enc.encode_mean(bk_px[lo:hi].contiguous()).to(dtype)
+            bk_mean = _all_gather_rows(mine, world, group)[:n_bk]
+        elif n_bk <= 4:
             # animate mode: the reference image and the (deduplicated) background go through the encoder together
             # (per-image arithmetic: the same values as two calls, one kernel chain instead of two)
             both = enc.encode_mean(torch.cat([ref_px, bk_px]))
             ref_latents, bk_mean = both[:1] * 0.18215, both[1:]
         else:
-            ref_latents, bk_mean = enc.encode_mean(ref_px) * 0.18215, None  # :424-431
-        if bk_mean is not None:
-            pass
-        elif world > 1 and n_bk >= world:
-            # edit mode: one distinct background per frame (run_edit.py:232-238) - every GPU encodes its share, one
-            # all-gather per clip (per-image arithmetic: identical to encoding them all here)
-            import torch.distributed as dist
-            per = -(-n_bk // world)
-            lo, hi = min(rank * per, n_bk), min((rank + 1) * per, n_bk)
-            mine = torch.zeros((per, 4, h, w), device=device, dtype=dtype)
-            if hi > lo:
-                mine[:hi - lo] = enc.encode_mean(bk_px[lo:hi].contiguous()).to(dtype)
-            every = torch.empty((world * per, 4, h, w), device=device, dtype=dtype)
-            dist.all_gather_into_tensor(every, mine, group=group)
-            bk_mean = every[:n_bk]
-        else:
-            bk_mean = enc.encode_mean(bk_px)
-        bk_lat = (bk_mean * 0.18215)[inp["bk_inverse"].to(device)]
-        vid_bk = bk_lat.permute(1, 0, 2, 3).unsqueeze(0).to(dtype).contiguous()  # [1, 4, F, h, w]  :434-443
-        mark("vae_encode")
+            ref_latents, bk_mean = enc.encode_mean(ref_px) * 0.18215, enc.encode_mean(bk_px)
+        bk_lat = (bk_mean * 0.18215)[inp["bk_inverse"].to(self.device)]
+        return ref_latents, bk_lat.permute(1, 0, 2, 3).unsqueeze(0).to(dtype).contiguous(), pose_px  # :434-443
 
-        if world > 1:
-            import torch.distributed as dist
-            if F_ % world == 0:  # pose features: each rank computes its frames, then all-gather [F, hw, 320]
-                fl = F_ // world
-                loc = self.pose_guider.forward_nhwc(pose_px[:, :, rank * fl:(rank + 1) * fl].contiguous())
-                pose_all = torch.empty((world * loc.shape[0], loc.shape[1]), dtype=loc.dtype, device=device)
-                dist.all_gather_into_tensor(pose_all, loc.contiguous(), group=group)
-                pose_fea = pose_all.reshape(F_, h * w, -1)
-            else:
-                pose_fea = self.pose_guider.forward_nhwc(pose_px).reshape(F_, h * w, -1)
-        else:
-            pose_fea = self.pose_guider.forward_nhwc(pose_px).reshape(F_, h * w, -1)  # channels-last, per frame
-        mark("pose_guider")
+    def _pose_features(self, pose_px: torch.Tensor, F_: int, h: int, w: int) -> torch.Tensor:
+        """Channels-last pose features [F, h * w, C]; ranks that divide F compute their frames and all-gather."""
+        rank, world, group = self._shard
+        if world > 1 and F_ % world == 0:
+            fl = F_ // world
+            loc = self.pose_guider.forward_nhwc(pose_px[:, :, rank * fl:(rank + 1) * fl].contiguous())
+            return _all_gather_rows(loc, world, group).reshape(F_, h * w, -1)
+        return self.pose_guider.forward_nhwc(pose_px).reshape(F_, h * w, -1)
 
-        context_scheduler = get_context_scheduler(context_schedule)
-        windows = list(context_scheduler(0, num_inference_steps, F_, context_frames, context_stride, context_overlap))
-        rep = 2 if do_cfg else 1
-        single = len(windows) == 1
-        plan = None
-        if world > 1:
-            from .shard import ShardPlan
-            if len({len(c) for c in windows}) != 1:
-                raise NotImplementedError("context windows of different lengths cannot be sharded")
-            plan = ShardPlan.make(world, rank, do_cfg, len(windows), len(windows[0]),
-                                  min_tokens=shard_tokens(h, w, len(self.denoising_unet.config.block_out_channels)))
-            forced = getattr(self, "force_plan", None)  # (cfg_ways, win_ways, frame_ways): tests exercise every axis
-            if forced is not None:
-                assert forced[0] * forced[1] * forced[2] == world
-                plan = ShardPlan(world, rank, *forced)
-        branches = plan.branches(do_cfg) if plan else tuple(range(rep))
-        nb = len(branches)
+    def _shard_plan(self, windows, do_cfg: bool, h: int, w: int):
+        """How the ranks divide the clip (host/shard.py: CFG branches x windows x frames), or None on one GPU."""
+        rank, world, _ = self._shard
+        if world <= 1:
+            return None
+        if len({len(c) for c in windows}) != 1:
+            raise NotImplementedError("context windows of different lengths cannot be sharded")
+        plan = ShardPlan.make(world, rank, do_cfg, len(windows), len(windows[0]),
+                              min_tokens=shard_tokens(h, w, len(self.denoising_unet.config.block_out_channels)))
+        if self.force_plan is not None:
+            assert self.force_plan[0] * self.force_plan[1] * self.force_plan[2] == world
+            plan = ShardPlan(world, rank, *self.force_plan)
+        return plan
 
-        # reference UNet once, banks -> denoising engine (pipeline :393-406, :480-490)
+    def _reference_pass(self, ref_latents, ehs, do_cfg: bool, branches, dtype):
+        """Reference UNet once, banks -> denoising engine for this GPU's CFG `branches` (pipeline :393-406, :480-490)."""
         writer = ReferenceAttentionControl(self.reference_unet, do_classifier_free_guidance=do_cfg, mode="write",
                                            batch_size=1, fusion_blocks="full")
         reader = ReferenceAttentionControl(self.denoising_unet, do_classifier_free_guidance=do_cfg, mode="read",
                                            batch_size=1, fusion_blocks="full")
         self.reference_unet(ref_latents.to(dtype).repeat(2 if do_cfg else 1, 1, 1, 1), torch.zeros((), dtype=torch.int64),
                             encoder_hidden_states=ehs, return_dict=False)
-        self.denoising_unet._branches = branches  # the CFG branch(es) this GPU evaluates
+        self.denoising_unet._branches = branches
         reader.update(writer)
-        den = self.denoising_unet.engine()
-        mark("reference_unet")
+        return reader, writer
 
+    def _denoise(self, sched, timesteps, latents, windows, plan, branches, pose_fea, vid_bk, guidance_scale: float,
+                 eta: float, step_noise, callback, callback_steps: int) -> None:
+        """The denoising loop (pipeline :492-561) on `latents`, in place: per step, this GPU's windows, then fused_step."""
+        device, dtype = self.device, latents.dtype
+        F_, h, w = latents.shape[2:]
+        do_cfg = guidance_scale > 1.0
+        rep, nb, single = 2 if do_cfg else 1, len(branches), len(windows) == 1
+        den = self.denoising_unet.engine()
         my_windows = plan.windows_of(len(windows)) if plan else list(range(len(windows)))
         win_inputs = []
         for wi in my_windows:  # the windows and their pose features are the same at every step (pipeline :493-500)
@@ -559,29 +578,25 @@ class Pose2VideoPipeline:
             fl = len(win_inputs[0][1])
             den.xchg, xw = self._exchanges(plan, nb, len(my_windows), fl, h, w, dtype)
             stages = [xw.bufs[k].view(len(my_windows), nb * 4 * fl * h * w, dtype) for k in ("S0", "S1")]
-            stage = stages[0]
-            gathered = torch.empty((world, len(my_windows), nb, 4, fl, h, w), dtype=dtype, device=device)
-            gcols = next(c for c in (64, 32, 16, 8) if stage.numel() % c == 0)
-            from .shard import gather_layout
+            gathered = torch.empty((plan.world, len(my_windows), nb, 4, fl, h, w), dtype=dtype, device=device)
+            gcols = next(c for c in (64, 32, 16, 8) if stages[0].numel() % c == 0)
             scatter = [(q, j, list(brs), torch.tensor(fr, dtype=torch.long, device=device))
                        for q, j, brs, fr in gather_layout(plan, windows, do_cfg)]
             counter_all = torch.zeros((F_,), device=device, dtype=dtype)
             for c in windows:
                 counter_all[c] = counter_all[c] + 1
-        else:
-            if den.xchg is not None:
-                den._graphs.clear()  # graphs captured with exchange nodes must not serve an un-sharded run
+        elif den.xchg is not None:
+            den._graphs.clear()  # graphs captured with exchange nodes must not serve an un-sharded run
             den.xchg = None
-        # multistep solvers: the model quantity m of the last two steps, slot i % 2 written at step i (every rank of a
-        # sharded run holds the whole clip's latents and keeps its own identical ring)
-        ring = None if ddim else torch.empty((2,) + tuple(latents.shape), dtype=dtype, device=device)
+        history = sched.new_history(latents)
+        draws = sched.step_draws(eta)
         for i, t in enumerate(timesteps):
             # scale_model_input (pipeline :519-521): the reference's own expression `x / s` with s a 0-dim fp32 tensor
             # for Euler; the identity for DDIM and DPM-Solver++
-            s_in = None if ddim else sched.model_input_scale(i)
+            s_in = sched.model_input_scale(i)
             lat_src = latents if s_in is None else latents / s_in
             if plan:
-                par = getattr(xw, "parity", 0)  # alternates across steps AND clips
+                par = xw.parity  # alternates across steps AND clips
                 xw.parity = par ^ 1
                 stage = stages[par]
                 for j, (c, cl, bk_c, pose_in) in enumerate(win_inputs):
@@ -607,54 +622,28 @@ class Pose2VideoPipeline:
             # the reference divides the window sums by `counter` only inside its guidance branch (pipeline :545-549):
             # without CFG, frames that two windows cover keep the SUM of both predictions - mirrored, not repaired
             pc, g_, cnt = (noise_pred[1], guidance_scale, counter) if do_cfg else (noise_pred[0], 1.0, None)
-            if not ddim:
-                co = sched.multistep_coefficients(i)
-                noise = None
-                if draws:  # Euler-ancestral: one draw per step, also at the last one (sigma_up = 0 there)
-                    noise = (step_noise[i] if step_noise is not None
-                             else torch.randn(tuple(latents.shape), device=device, dtype=dtype))
-                ops.cfg_multistep(noise_pred[0], pc, latents, g_, co, ring[i % 2],
-                                  h1=ring[(i - 1) % 2] if co[4] != 0 else None, h2=ring[i % 2] if co[5] != 0 else None,
-                                  noise=noise if co[6] != 0 else None, counter=cnt, frame_stride=h * w)
-            elif eta > 0:
-                co = sched.step_coefficients(t)
-                # DDIMScheduler.step [3P] draws its noise at every step, also the last one (sigma = 0 there)
-                dir_c, sigma = sched.noise_coefficients(t, eta)
+            noise = None
+            if draws:  # one draw per step, also at the last one where its coefficient is 0 (DDIMScheduler.step [3P])
                 noise = (step_noise[i] if step_noise is not None
                          else torch.randn(tuple(latents.shape), device=device, dtype=dtype))
-                ops.cfg_ddim_step_noise(noise_pred[0], pc, latents, g_, *co[:3], dir_c, noise, sigma, counter=cnt,
-                                        frame_stride=h * w)
-            else:
-                co = sched.step_coefficients(t)
-                ops.cfg_ddim_step(noise_pred[0], pc, latents, g_, *co, counter=cnt, frame_stride=h * w)
+            sched.fused_step(i, t, noise_pred[0], pc, latents, g_, eta=eta, noise=noise, history=history, counter=cnt,
+                             frame_stride=h * w)
             # the reference's inner `for i in range(num_context_batches)` (pipeline :503-510) shadows the step index: its
             # callback test (:556-561) and the index it passes see the LAST CONTEXT BATCH's index, at every step
             i_ref = len(windows) - 1
             if callback is not None and i_ref % callback_steps == 0:
                 callback(i_ref, t, latents)
-        mark("denoise")
-        reader.clear()
-        writer.clear()
-        out = {"latents": latents}
-        if decode:
-            vid_lat = latents
-            if interp is not None:  # pipeline :566-567: the frames to decode, (F - 1) * k + 1 of them
-                vid_lat = ops.interpolate_frames(latents, interpolation_factor, interp)
-                mark("interpolate")
-            Fv = vid_lat.shape[2]
-            if world > 1 and Fv % world == 0:
-                fl = Fv // world
-                loc = self.decode_latents_device(vid_lat[:, :, rank * fl:(rank + 1) * fl])  # [1, 3, fl, H, W]
-                parts = torch.empty((world * loc.shape[0],) + tuple(loc.shape[1:]), dtype=loc.dtype, device=device)
-                dist.all_gather_into_tensor(parts, loc.contiguous(), group=group)
-                out["videos"] = parts.view((world,) + tuple(loc.shape)).permute(1, 2, 0, 3, 4, 5).reshape(
-                    1, 3, Fv, loc.shape[-2], loc.shape[-1])
-            else:
-                out["videos"] = self.decode_latents_device(vid_lat)
-            mark("vae_decode")
-        self._marks = marks
-        self.last_latents = latents
-        return out
+
+    def _decode(self, vid_lat: torch.Tensor) -> torch.Tensor:
+        """decode_latents_device(); ranks that divide the frames decode their frames and all-gather."""
+        rank, world, group = self._shard
+        Fv = vid_lat.shape[2]
+        if world > 1 and Fv % world == 0:
+            fl = Fv // world
+            loc = self.decode_latents_device(vid_lat[:, :, rank * fl:(rank + 1) * fl])  # [1, 3, fl, H, W]
+            return _all_gather_rows(loc, world, group).view((world,) + tuple(loc.shape)).permute(1, 2, 0, 3, 4, 5).reshape(
+                1, 3, Fv, loc.shape[-2], loc.shape[-1])
+        return self.decode_latents_device(vid_lat)
 
     def _collect_timings(self):
         m = self._marks
@@ -680,7 +669,6 @@ class Pose2VideoPipeline:
         self._interpolation_method(interpolation_factor, video_length)  # before any work is done
         dtype = self.denoising_unet.dtype
         self.latent_levels(width, height)  # refuses only images smaller than one latent pixel
-        from .scheduler import engine_scheduler
         engine_scheduler(self.scheduler)  # refuses LMS, PNDM and unknown schedulers before any work
         host = self.preprocess(ref_image, pose_images, vid_bk_images, width, height, video_length, generator, dtype,
                                num_inference_steps, eta)

@@ -4,10 +4,10 @@ The reference builds `diffusers.DDIMScheduler(**noise_scheduler_kwargs)` (run_an
 configs/inference/inference_v2.yaml:24-33) and its pipeline accepts six diffusers scheduler classes (pipeline :11-18,
 :46-53); diffusers is a third-party dependency that is not part of the reference tree. The classes here accept the same
 keyword arguments, expose what the pipeline touches (set_timesteps / timesteps / init_noise_sigma / scale_model_input /
-order / alphas_cumprod / config / a tensor step()) and, for the engine's sampler, the scalars of its fused kernels:
-DDIMScheduler.step_coefficients for mimo_cfg_ddim_step, multistep_coefficients(i) of the other three for
-mimo_cfg_multistep. The DDIM integer tables are pinned by tests/golden/integer_tables.json. engine_scheduler() maps a
-caller's scheduler (an engine one, or a diffusers instance read as a config container) to the engine's class.
+order / alphas_cumprod / config / a tensor step()) and, for the engine's sampler, fused_step(): DDIM runs
+mimo_cfg_ddim_step(_noise), the other three mimo_cfg_multistep with multistep_coefficients(i). The DDIM integer tables
+are pinned by tests/golden/integer_tables.json. engine_scheduler() maps a caller's scheduler (an engine one, or a
+diffusers instance read as a config container) to the engine's class.
 """
 from __future__ import annotations
 
@@ -17,6 +17,8 @@ from types import SimpleNamespace
 
 import numpy as np
 import torch
+
+from .. import ops
 
 
 def _betas(name: str, num_train_timesteps: int, beta_start: float, beta_end: float, beta_schedule: str,
@@ -46,15 +48,31 @@ def _check_v_prediction(prediction_type: str) -> None:
                                   "inference_v2.yaml) is implemented")
 
 
-def _config(config) -> dict:
-    """A scheduler config (dict / diffusers FrozenDict / namespace) as a dict without diffusers' private `_` keys."""
-    items = config.items() if isinstance(config, Mapping) else vars(config).items()
-    return {k: v for k, v in items if not k.startswith("_")}
-
-
-class DDIMScheduler:
+class _Scheduler:
+    """What the schedulers the engine runs share. The sampler loop (Pose2VideoPipeline._denoise) calls new_history()
+    and step_draws() once per clip, then model_input_scale(i) and fused_step() at every step i."""
     order = 1
 
+    @classmethod
+    def from_config(cls, config, **overrides):
+        items = config.items() if isinstance(config, Mapping) else vars(config).items()
+        return cls(**{**{k: v for k, v in items if not k.startswith("_")}, **overrides})
+
+    def scale_model_input(self, sample, timestep=None):
+        return sample
+
+    @staticmethod
+    def _step_output(prev, x0, return_dict: bool):
+        return SimpleNamespace(prev_sample=prev, pred_original_sample=x0) if return_dict else (prev,)
+
+    def model_input_scale(self, i: int):
+        return None  # the divisor scale_model_input applies at step i; None: the identity
+
+    def new_history(self, latents: torch.Tensor):
+        return None  # what fused_step() carries from one step of a clip to the next
+
+
+class DDIMScheduler(_Scheduler):
     def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.0001, beta_end: float = 0.02,
                  beta_schedule: str = "linear", clip_sample: bool = True, set_alpha_to_one: bool = True,
                  steps_offset: int = 0, prediction_type: str = "epsilon", rescale_betas_zero_snr: bool = False,
@@ -73,12 +91,7 @@ class DDIMScheduler:
                                       set_alpha_to_one=set_alpha_to_one, steps_offset=steps_offset,
                                       prediction_type=prediction_type, rescale_betas_zero_snr=rescale_betas_zero_snr,
                                       timestep_spacing=timestep_spacing)
-        self.num_inference_steps = None
-        self.timesteps = None
-
-    @classmethod
-    def from_config(cls, config, **overrides):
-        return cls(**{**_config(config), **overrides})
+        self.num_inference_steps = self.timesteps = None
 
     def set_timesteps(self, num_inference_steps: int, device=None):
         T = self.config.num_train_timesteps
@@ -95,16 +108,13 @@ class DDIMScheduler:
             raise ValueError(f"{sp} is not supported")
         self.timesteps = torch.from_numpy(ts).to(device)
 
-    def scale_model_input(self, sample, timestep=None):
-        return sample
-
     def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, eta: float = 0.0,
              use_clipped_model_output: bool = False, generator=None, variance_noise=None, return_dict: bool = True,
              **unused):
         """diffusers DDIMScheduler.step [3P] for v-prediction (pipeline :128-147, :551-553): tensor in, tensor out, in
         the dtype / on the device of `sample`. eta > 0 adds sigma * noise, the noise being `variance_noise` or drawn by
         randn_tensor(model_output.shape, generator, dtype=model_output.dtype) - at every call, also at the last step
-        where sigma = 0. The engine's own sampler uses the fused kernels (step_coefficients / noise_coefficients);
+        where sigma = 0. The engine's own sampler runs fused_step() (step_coefficients / noise_coefficients);
         this method exists so that the reference's unmodified pipeline file runs over this scheduler."""
         if self.num_inference_steps is None:
             raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating "
@@ -132,16 +142,12 @@ class DDIMScheduler:
         else:
             direction = (1 - a_p) ** 0.5 * eps  # std_dev_t = 0 at eta = 0
             prev = a_p ** 0.5 * x0 + direction
-        if not return_dict:
-            return (prev,)
-        return SimpleNamespace(prev_sample=prev, pred_original_sample=x0)
+        return self._step_output(prev, x0, return_dict)
 
     def step_coefficients(self, t: int):
         """(sqrt(abar_t), sqrt(1 - abar_t), sqrt(abar_prev), sqrt(1 - abar_prev)); prev_t = t - T // N (NOT the next
         table entry: for N = 30 they differ)."""
-        prev_t = t - self.config.num_train_timesteps // self.num_inference_steps
-        a_t = self.alphas_cumprod[t]
-        a_p = self.alphas_cumprod[prev_t] if prev_t >= 0 else self.final_alpha_cumprod
+        a_t, a_p = self._alphas(t)
         return float(a_t ** 0.5), float((1 - a_t) ** 0.5), float(a_p ** 0.5), float((1 - a_p) ** 0.5)
 
     def _alphas(self, t: int):
@@ -169,11 +175,24 @@ class DDIMScheduler:
         std_dev_t = eta * self._variance(a_t, a_p) ** 0.5
         return float(self._direction(a_p, std_dev_t)), float(std_dev_t)
 
+    def step_draws(self, eta: float) -> bool:
+        return eta > 0  # step() draws randn_tensor(model_output.shape) at every step, also the last one
+
+    def fused_step(self, i, t, pred_uncond, pred_cond, latents, guidance, *, eta, noise, history, counter, frame_stride):
+        """CFG + DDIM step at timestep t, on `latents` in place; eta > 0 adds sigma * noise."""
+        co = self.step_coefficients(t)
+        if eta > 0:
+            dir_c, sigma = self.noise_coefficients(t, eta)
+            ops.cfg_ddim_step_noise(pred_uncond, pred_cond, latents, guidance, *co[:3], dir_c, noise, sigma,
+                                    counter=counter, frame_stride=frame_stride)
+        else:
+            ops.cfg_ddim_step(pred_uncond, pred_cond, latents, guidance, *co, counter=counter, frame_stride=frame_stride)
+
 
 # ------------------------------------------------------------------------------------------------
 # DPM-Solver++ multistep, Euler and Euler-ancestral
 # ------------------------------------------------------------------------------------------------
-class _SigmaScheduler:
+class _SigmaScheduler(_Scheduler):
     """What the three non-DDIM schedulers share: DDIMScheduler's betas and abar, except that with
     rescale_betas_zero_snr abar at the last timestep is 2^-24 instead of 0 (so sigma_max = sqrt((1 - abar) / abar) is
     about 4096, not infinite), step-index bookkeeping, and the affine form of a step that mimo_cfg_multistep runs:
@@ -184,7 +203,6 @@ class _SigmaScheduler:
     with v the guided v-prediction, h_1 / h_2 the m of the previous two steps and noise this step's draw.
     multistep_coefficients(i) gives (a, b, c_x, c_m, c_1, c_2, c_n) for step i in float64 (from the fp32 abar / sigma
     tables), which the caller casts to fp32 once."""
-    order = 1
     draws_noise = False  # whether step() consumes one randn draw of the sample's shape per step
 
     def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.0001, beta_end: float = 0.02,
@@ -204,13 +222,7 @@ class _SigmaScheduler:
                                       beta_end=beta_end, beta_schedule=beta_schedule, prediction_type=prediction_type,
                                       rescale_betas_zero_snr=rescale_betas_zero_snr,
                                       timestep_spacing=timestep_spacing, steps_offset=steps_offset)
-        self.num_inference_steps = None
-        self.timesteps = None
-        self._step_index = None
-
-    @classmethod
-    def from_config(cls, config, **overrides):
-        return cls(**{**_config(config), **overrides})
+        self.num_inference_steps = self.timesteps = self._step_index = None
 
     @property
     def step_index(self):
@@ -236,12 +248,19 @@ class _SigmaScheduler:
         """sqrt((1 - abar) / abar) over the training timesteps, in fp32 as diffusers computes it."""
         return (((1 - self.alphas_cumprod) / self.alphas_cumprod) ** 0.5).numpy()
 
-    def model_input_scale(self, i: int):
-        """The divisor scale_model_input applies at step i, or None where it is the identity."""
-        return None
+    def step_draws(self, eta: float) -> bool:
+        return self.draws_noise  # eta reaches DDIM only (prepare_extra_step_kwargs, pipeline :128-147)
 
-    def multistep_coefficients(self, i: int):
-        raise NotImplementedError
+    def new_history(self, latents: torch.Tensor) -> torch.Tensor:
+        """The m of the last two steps, slot i % 2 written at step i (every rank of a sharded run keeps its own)."""
+        return torch.empty((2,) + tuple(latents.shape), dtype=latents.dtype, device=latents.device)
+
+    def fused_step(self, i, t, pred_uncond, pred_cond, latents, guidance, *, eta, noise, history, counter, frame_stride):
+        """CFG + step i, on `latents` in place; h_1, h_2 and the noise are passed where their coefficient is not 0."""
+        co = self.multistep_coefficients(i)
+        ops.cfg_multistep(pred_uncond, pred_cond, latents, guidance, co, history[i % 2],
+                          h1=history[(i - 1) % 2] if co[4] != 0 else None, h2=history[i % 2] if co[5] != 0 else None,
+                          noise=noise if co[6] != 0 else None, counter=counter, frame_stride=frame_stride)
 
 
 class DPMSolverMultistepScheduler(_SigmaScheduler):
@@ -299,9 +318,6 @@ class DPMSolverMultistepScheduler(_SigmaScheduler):
         self.num_inference_steps = len(ts)
         self.model_outputs = [None] * self.config.solver_order
         self._step_index = None
-
-    def scale_model_input(self, sample, timestep=None):
-        return sample
 
     def _vp(self, i: int):
         """(alpha, sigma, lambda) at table position i in float64; i = N is the final sigma = 0 (abar = 1)."""
@@ -378,9 +394,7 @@ class DPMSolverMultistepScheduler(_SigmaScheduler):
             prev = (cx * sample - A * m0 + (at * ((eh - 1.0) / h + 1.0)) * D1
                     - (at * ((eh - 1.0 + h) / h ** 2 - 0.5)) * D2)
         self._step_index += 1
-        if not return_dict:
-            return (prev,)
-        return SimpleNamespace(prev_sample=prev, pred_original_sample=x0)
+        return self._step_output(prev, x0, return_dict)
 
 
 class EulerDiscreteScheduler(_SigmaScheduler):
@@ -474,9 +488,7 @@ class EulerDiscreteScheduler(_SigmaScheduler):
         if noise is not None:
             prev = prev + noise * up
         self._step_index += 1
-        if not return_dict:
-            return (prev,)
-        return SimpleNamespace(prev_sample=prev, pred_original_sample=x0)
+        return self._step_output(prev, x0, return_dict)
 
 
 class EulerAncestralDiscreteScheduler(EulerDiscreteScheduler):
@@ -527,7 +539,7 @@ def engine_scheduler(obj):
     """The engine's scheduler for the caller's `obj`: an engine scheduler is returned as it is; anything else is read as
     a config container, as a diffusers scheduler is: the engine class of the same name is built from `obj.config`
     (its `_`-prefixed keys dropped). LMS, PNDM and unknown classes are refused."""
-    if isinstance(obj, (DDIMScheduler, _SigmaScheduler)):
+    if isinstance(obj, _Scheduler):
         return obj
     name = type(obj).__name__
     cls = _ALL.get(name)

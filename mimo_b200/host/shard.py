@@ -174,6 +174,7 @@ class Exchange:
         self.G, self.r, self.flags, self.bufs, self.device = G, r, flags, bufs, device
         self.ctl = torch.tensor([1, 0], dtype=torch.int32, device=device)
         self.timeout_ms, self.max_blocks = timeout_ms, max_blocks
+        self.parity = 0  # which of the two all-gather sources (S0 / S1) the sampler writes next
 
     @staticmethod
     def local_group(G: int, sizes: Dict[str, int], device, **kw) -> List["Exchange"]:
