@@ -41,7 +41,8 @@ const char* mimo_last_error(void);
 /* 0 if device `dev` is sm_90; MIMO_ERR_DEVICE otherwise (also when there is no CUDA device at all). */
 int mimo_device_check(int dev);
 /* sizeof() of the parameter structs as compiled into the library (0 epilogue, 1 gemm, 2 conv3x3, 3 groupnorm,
- * 4 attn, 5 attn_temporal, 6 exchange, 7 cfg_multistep, 8 groupnorm_window): lets a binding verify its struct mirrors
+ * 4 attn, 5 attn_temporal, 6 exchange, 7 cfg_multistep, 8 groupnorm_window, 9 gemm_e4m3): lets a binding verify its
+ * struct mirrors
  * before the first call. */
 int mimo_abi_sizeof(int which);
 
@@ -87,6 +88,33 @@ typedef struct {
 int mimo_gemm(const mimo_gemm_params* p, void* stream);
 /* number of value rows (== gate rows) per packed GEGLU tile for a packed width N (N = 2 * out features) */
 int mimo_gemm_geglu_granule(int32_t N);
+
+/* FP8 form of mimo_gemm for projections fed by mimo_layernorm_e4m3:
+ *   out[M,N] = epilogue((A[M,K] . W[N,K]^T)[m][n] * a_scale[m] * w_scale[n])
+ * A and W are e4m3 (OCP E4M3FN, one byte per element, both K-major), a_scale / w_scale fp32; accumulation in fp32. The
+ * product with the two scales is taken in fp32 in that order, then the mimo_epilogue chain runs as in mimo_gemm (bias,
+ * residual, act NONE or GEGLU, scale); out, bias, rowvec and residual are `dtype` (fp16 / bf16).
+ * Replaces, when the caller opts into FP8: the q|k|v projection after norm1 (src/models/attention.py:329-345 ->
+ * mutual_self_attention.py:154-197), the GEGLU up-projection after norm3 (attention.py:359-360), and the motion module's
+ * q|k|v after its norms + PE (motion_module.py:230, 277-292) and its GEGLU after ff_norm (motion_module.py:235-236).
+ * Requirements: GEMM rows only (no second A source, no split-K: workspace must be NULL), K % 16 == 0, lda / ldw % 16 == 0
+ * (bytes), N % 8 == 0, ldo % 8 == 0, 16-byte aligned a / w / out / residual, non-NULL scales; GEGLU needs N % 256 == 0. */
+typedef struct {
+  const void* a;        /* [M, lda] e4m3 */
+  int64_t lda;
+  const float* a_scale; /* [M] */
+  const void* w;        /* [N, ldw] e4m3 (GEGLU: packed as for mimo_gemm) */
+  int64_t ldw;
+  const float* w_scale; /* [N] */
+  void* out;
+  int64_t ldo;
+  int32_t M, N, K;
+  int32_t dtype; /* of out / bias / rowvec / residual */
+  mimo_epilogue ep;
+  void* workspace; /* must be NULL (split-K is not supported in e4m3) */
+  int64_t workspace_bytes;
+} mimo_gemm_e4m3_params;
+int mimo_gemm_e4m3(const mimo_gemm_e4m3_params* p, void* stream);
 
 /* 3x3 / stride 1 / pad 1 convolution as implicit GEMM: the A operand is fetched tap by tap with 4-D TMA boxes
  * over the NHWC input (out-of-bounds = zero padding), optionally from two tensors (virtual channel concat).
@@ -190,6 +218,15 @@ int64_t mimo_groupnorm_window_table_bytes(const mimo_groupnorm_window_params* p)
 int mimo_layernorm(const void* x, const void* gamma, const void* beta, void* out, int64_t rows, int32_t c,
                    float eps, const void* pe, int64_t rows_per_frame, int32_t frames, int32_t pe_frame_offset,
                    int32_t dtype, void* stream);
+/* mimo_layernorm with an e4m3 output and one fp32 scale per row: the A operand of mimo_gemm_e4m3. With y the row's fp32
+ * LN(+PE) values (with a PE, LN's output is rounded to `dtype` before the encoding is added, as in mimo_layernorm):
+ *   amax = max |y|;  inv = 448 / amax, scale[r] = amax / 448 (IEEE divisions);  out[r] = cvt.rn.satfinite.e4m3(y * inv)
+ * and inv = scale[r] = 1 when amax == 0. out is [rows, c] bytes, scale [rows] fp32; x, gamma, beta, pe are `dtype`.
+ * Replaces, when the caller opts into FP8, the nn.LayerNorm (+ PositionalEncoding) call sites ahead of mimo_gemm_e4m3's
+ * projections (attention.py:329-360; motion_module.py:230, 236, 277-279). Requirements as mimo_layernorm, and c % 16 == 0. */
+int mimo_layernorm_e4m3(const void* x, const void* gamma, const void* beta, void* out, float* scale, int64_t rows,
+                        int32_t c, float eps, const void* pe, int64_t rows_per_frame, int32_t frames,
+                        int32_t pe_frame_offset, int32_t dtype, void* stream);
 
 /* Spatial self-attention with the reference-image bank (flash attention, wgmma QK^T and PV, online softmax).
  * q/k/v: [n, lq, heads, d] slices of a fused QKV buffer (row stride ld_qkv elements). bank_k/bank_v:

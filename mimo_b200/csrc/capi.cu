@@ -71,8 +71,9 @@ int encode_tmap(CUtensorMap* out, int dtype, int rank, const void* base, const u
     es[i] = 1;
     if (i + 1 < rank) gstr[i] = strides_bytes[i];
   }
-  const CUtensorMapDataType dt =
-      dtype == MIMO_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const CUtensorMapDataType dt = dtype == kTmapU8     ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                 : dtype == MIMO_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                      : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   CUresult r = g_encode(out, dt, static_cast<cuuint32_t>(rank), const_cast<void*>(base), gdim, gstr, bx, es,
                         CU_TENSOR_MAP_INTERLEAVE_NONE,
                         swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
@@ -107,6 +108,7 @@ extern "C" int mimo_abi_sizeof(int which) {
     case 6: return static_cast<int>(sizeof(mimo_exchange_params));
     case 7: return static_cast<int>(sizeof(mimo_cfg_multistep_params));
     case 8: return static_cast<int>(sizeof(mimo_groupnorm_window_params));
+    case 9: return static_cast<int>(sizeof(mimo_gemm_e4m3_params));
   }
   return -1;
 }

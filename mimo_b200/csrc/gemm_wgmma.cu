@@ -18,6 +18,9 @@
 // (tap, 64-channel block, source tensor); TMA's out-of-bounds zero fill is the conv's zero padding and also
 // the K tail, and the output / residual boxes use the same {TW, TH, TN} footprint (stores are clipped at image
 // borders). Two source tensors give the up-blocks' channel concat without materialising it.
+// E4M3 mode (mimo_gemm_e4m3, GEMM rows only) runs the same roles on fp8 A and W: a K block is 128 one-byte elements, the
+// same 128-byte swizzle row and stage bytes, four wgmma.m64nBNk32.e4m3 per block; the epilogue first takes
+// acc * a_scale[row] * w_scale[col] in fp32 and then runs the chain above unchanged.
 #include <cuda_runtime.h>
 
 #include <cudaTypedefs.h>
@@ -60,7 +63,7 @@ struct ConvGeom {
   signed char tdx[9], tdy[9];  // input offset of tap t relative to the output pixel
 };
 
-template <int BN, bool kRes>
+template <int BN, bool kRes, bool kE4m3 = false>
 struct GemmCfg {
   static constexpr int kStageBytes = BM * BK * 2 + BN * BK * 2;
   static constexpr int kNChunk = BN / 32;
@@ -68,7 +71,9 @@ struct GemmCfg {
   static constexpr int kResSlots = kRes ? 2 : 0;
   static constexpr int kResBytes = kResSlots * kChunk;
   static constexpr int kBarBytes = 512;
-  static constexpr int kFixed = kBarBytes + 2048 /*sbias*/ + kOutBytes + kResBytes;
+  // e4m3 adds [2][256] column and [2][128] row scales (3 KiB). At BN = 256 with a residual that leaves room for 3 stages
+  // instead of 4; the engine's e4m3 GEMMs (q|k|v, GEGLU) take no residual and keep 4.
+  static constexpr int kFixed = kBarBytes + 2048 /*sbias*/ + (kE4m3 ? 3072 /*column, row scales*/ : 0) + kOutBytes + kResBytes;
   static constexpr int kMaxStages = (BN >= 256) ? 4 : (BN >= 160 ? 5 : (BN >= 128 ? 6 : 8));
   static constexpr int kFit = (227 * 1024 - kFixed) / kStageBytes;
   static constexpr int kStages = kFit < kMaxStages ? kFit : kMaxStages;
@@ -83,376 +88,23 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
                   const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOut,
                   const __grid_constant__ CUtensorMap tmRes, int M, int N, int num_m_tiles, int num_n_tiles,
                   int num_k_blocks, ConvGeom g, EpiArgs ep) {
-  using Cfg = GemmCfg<BN, kRes>;
-  using C = Cvt<kBf16>;
-  using T = typename C::T;
-  constexpr int NCHUNK = Cfg::kNChunk;
-  extern __shared__ __align__(1024) uint8_t smem[];  // 128B-swizzled tiles need 1024-byte alignment
-  uint8_t* sOut = smem + Cfg::kStages * Cfg::kStageBytes;  // [2 buffers][8 KiB]
-  uint8_t* sRes = sOut + Cfg::kOutBytes;                    // [kResSlots][8 KiB]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sRes + Cfg::kResBytes);
-  uint64_t* full_bar = bars;        // kStages (<= 8)
-  uint64_t* empty_bar = bars + 8;   // kStages
-  uint64_t* res_full = bars + 16;   // kResSlots (<= 2)
-  uint64_t* res_empty = bars + 18;  // kResSlots
-  float* sbias = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + Cfg::kBarBytes);  // [2][256]
+  constexpr bool kE4m3 = false;
+  constexpr const float* a_scale = nullptr;
+  constexpr const float* w_scale = nullptr;
+#include "gemm_wgmma_body.cuh"
+}
 
-  pdl_launch_dependents();
-  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);  // provably warp-uniform for the compiler
-  const int lane = threadIdx.x & 31;
-  const int num_tiles = num_m_tiles * num_n_tiles * g.splits;
-  // tile -> (output tile, K range): with split-K several CTAs share an output tile and each takes kb_split K blocks
-  auto decode = [&](int tile, int& m_tile, int& n_tile, int& split, int& kb_begin, int& kb_cnt) {
-    const int mn = tile / g.splits;
-    split = tile - mn * g.splits;
-    m_tile = mn / num_n_tiles;
-    n_tile = mn - m_tile * num_n_tiles;
-    kb_begin = split * g.kb_split;
-    kb_cnt = num_k_blocks - kb_begin;
-    if (kb_cnt > g.kb_split) kb_cnt = g.kb_split;
-  };
-
-  if (warp == 8 && lane == 0) {
-    tma_prefetch_desc(&tmA0);
-    tma_prefetch_desc(&tmA1);
-    tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmOut);
-    if (kRes) tma_prefetch_desc(&tmRes);
-  }
-  if (warp == 9 && lane == 0) {
-    for (int s = 0; s < Cfg::kStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 8);  // lane 0 of each MMA warp, once its wgmma group has read the stage
-    }
-    for (int s = 0; s < Cfg::kResSlots; ++s) {
-      mbar_init(&res_full[s], 1);
-      mbar_init(&res_empty[s], 8);
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  pdl_wait();  // everything above touched only shared memory / the kernel parameters
-
-  // tile -> coordinates of its first output row / pixel
-  auto tile_origin = [&](int m_tile, int& x0, int& y0, int& n0) {
-    if (g.conv) {
-      x0 = (m_tile % g.tiles_w) * g.TW;
-      y0 = ((m_tile / g.tiles_w) % g.tiles_h) * g.TH;
-      n0 = (m_tile / (g.tiles_w * g.tiles_h)) * g.TN;
-    } else {
-      x0 = y0 = n0 = 0;
-    }
-  };
-
-  // Producer warps run their loops with all 32 lanes (uniform control flow) and elect one lane for the TMA
-  // instructions: addresses then live in uniform registers.
-  if (warp == 8) {
-    // ===================== TMA producer (operands) =====================
-    // (all index arithmetic is incremental: one division per tile, only under split-K)
-    uint32_t stage = 0, phase = 0;
-    const int kb_per_tap = g.kb0 + g.kb1;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      int m_tile, n_tile, split, kb_begin, kb_cnt;
-      decode(tile, m_tile, n_tile, split, kb_begin, kb_cnt);
-      int x0, y0, n0;
-      tile_origin(m_tile, x0, y0, n0);
-      // conv: k-block inside the tap, tap index / offsets, tap * ctot
-      int tap = kb_per_tap > 0 ? kb_begin / kb_per_tap : 0;
-      int rem = kb_begin - tap * kb_per_tap;
-      int dx = g.tdx[tap], dy = g.tdy[tap], tap_k = tap * g.ctot;
-      for (int kbl = 0, kb = kb_begin; kbl < kb_cnt; ++kbl, ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1u);
-        uint8_t* sa = smem + stage * Cfg::kStageBytes;
-        uint8_t* sb = sa + BM * BK * 2;
-        if (elect_one()) {
-          if (!g.conv) {
-            mbar_expect_tx(&full_bar[stage], BM * BK * 2 + BN * BK * 2);
-            if (kb < g.kb0) {  // A = [A0 | A1] along K (virtual concat for the up-block shortcut GEMMs)
-              tma_load_2d(sa, &tmA0, &full_bar[stage], kb * BK, m_tile * BM);
-              tma_load_2d(sb, &tmB, &full_bar[stage], kb * BK, n_tile * BN);
-            } else {
-              tma_load_2d(sa, &tmA1, &full_bar[stage], (kb - g.kb0) * BK, m_tile * BM);
-              tma_load_2d(sb, &tmB, &full_bar[stage], g.c0 + (kb - g.kb0) * BK, n_tile * BN);
-            }
-          } else {
-            mbar_expect_tx(&full_bar[stage], g.a_bytes + BN * BK * 2);
-            int kcoord;
-            if (rem < g.kb0) {
-              tma_load_4d(sa, &tmA0, &full_bar[stage], rem * BK, x0 + dx, y0 + dy, n0);
-              kcoord = tap_k + rem * BK;
-            } else {
-              tma_load_4d(sa, &tmA1, &full_bar[stage], (rem - g.kb0) * BK, x0 + dx, y0 + dy, n0);
-              kcoord = tap_k + g.c0 + (rem - g.kb0) * BK;
-            }
-            tma_load_2d(sb, &tmB, &full_bar[stage], kcoord, n_tile * BN);
-          }
-        }
-        __syncwarp();
-        if (++rem == kb_per_tap) {
-          rem = 0;
-          tap_k += g.ctot;
-          if (++tap == g.ntaps) tap = 0;
-          dx = g.tdx[tap];
-          dy = g.tdy[tap];
-        }
-        if (++stage == Cfg::kStages) {
-          stage = 0;
-          phase ^= 1u;
-        }
-      }
-    }
-  } else if (warp == 9) {
-    // ===================== TMA producer (residual chunks) =====================
-    if constexpr (kRes) {
-      uint32_t k = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m_tile = tile / num_n_tiles;  // (a residual never comes with split-K: splits == 1 here)
-        const int n_tile = tile % num_n_tiles;
-        int x0, y0, n0;
-        tile_origin(m_tile, x0, y0, n0);
-        for (int c = 0; c < NCHUNK; ++c, ++k) {
-          const uint32_t slot = k % Cfg::kResSlots;
-          mbar_wait(&res_empty[slot], ((k / Cfg::kResSlots) & 1u) ^ 1u);
-          if (elect_one()) {
-            mbar_expect_tx(&res_full[slot], g.chunk_bytes);
-            const int col = n_tile * BN + c * 32;  // boxes beyond N are zero-filled (keeps the slot sequence uniform)
-            if (g.conv)
-              tma_load_4d(sRes + slot * kChunk, &tmRes, &res_full[slot], col, x0, y0, n0);
-            else
-              tma_load_2d(sRes + slot * kChunk, &tmRes, &res_full[slot], col, m_tile * BM);
-          }
-          __syncwarp();
-        }
-      }
-    }
-  } else if (warp < 8) {
-    // ===================== MMA + epilogue (warpgroups 0, 1) =====================
-    const int wg = warp >> 2;    // tile rows [64 wg, 64 wg + 64)
-    const int ct = threadIdx.x;  // 0..255
-    // wgmma accumulator layout: warp w of the warpgroup holds rows 16 w + lane / 4 (+ 8); fragment j (8 columns)
-    // holds columns 8 j + 2 (lane % 4) (+ 1) in acc[4 j + {0, 1}] (row) and acc[4 j + {2, 3}] (row + 8)
-    const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-    const int q2 = (lane & 3) * 2;
-    const bool issuer = ct == 0;
-    const int sw[2] = {(rbase >> 1) & 3, ((rbase + 8) >> 1) & 3};  // 64-byte swizzle: 16-byte piece ^= addr bits [7:8]
-    const bool do_silu = ep.act == MIMO_ACT_SILU;
-    // (32-bit arithmetic: M, the pixel count and rows_per_group all fit an int; 64-bit divisions cost ~1 us here)
-    const uint32_t rpg = static_cast<uint32_t>(ep.rows_per_group);
-    float acc[BN / 2];
-    uint32_t stage = 0, phase = 0, lt = 0, oc = 0, rc = 0;
-
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++lt) {
-      int m_tile, n_tile, split, kb_begin, kb_cnt;
-      decode(tile, m_tile, n_tile, split, kb_begin, kb_cnt);
-      int x0, y0, n0;
-      tile_origin(m_tile, x0, y0, n0);
-      // first / last group touched by a tile (uniform per tile)
-      auto tile_groups = [&](int mt, uint32_t& gf, uint32_t& gl) {
-        if (!g.conv) {
-          const uint32_t m0 = static_cast<uint32_t>(mt) * BM;
-          uint32_t m1 = m0 + BM - 1;
-          if (m1 > static_cast<uint32_t>(M) - 1) m1 = static_cast<uint32_t>(M) - 1;
-          gf = m0 / rpg;
-          gl = m1 / rpg;
-        } else {
-          int tx, ty, tn;
-          tile_origin(mt, tx, ty, tn);
-          int n1 = tn + g.TN - 1;
-          if (n1 > g.NI - 1) n1 = g.NI - 1;
-          const uint32_t hw = static_cast<uint32_t>(g.H) * g.W;
-          gf = (static_cast<uint32_t>(tn) * hw) / rpg;
-          gl = (static_cast<uint32_t>(n1 + 1) * hw - 1) / rpg;
-        }
-      };
-      // column constants of a tile: bias (+ the per-branch vector when the whole tile shares one group)
-      const int ce = ct;  // one column per MMA-warpgroup thread (BN <= 256)
-      auto load_consts = [&](int t) -> float {
-        float v = 0.f;
-        const int mt = (t / g.splits) / num_n_tiles, nt = (t / g.splits) % num_n_tiles;
-        const int col = nt * BN + ce;
-        if (ce < BN && col < N) {
-          if (ep.bias) v = C::to_f(static_cast<const T*>(ep.bias)[col]);
-          if (ep.rowvec) {
-            uint32_t gf, gl;
-            tile_groups(mt, gf, gl);
-            if (gf == gl) v += C::to_f(static_cast<const T*>(ep.rowvec)[static_cast<long long>(gf) * ep.ld_rowvec + col]);
-          }
-        }
-        return ep.act == MIMO_ACT_GEGLU ? v : v * ep.scale;  // y = acc * scale + (bias + vec) * scale
-      };
-      float* sb = sbias + (lt & 1u) * 256;
-      if (ct < BN) sb[ct] = load_consts(tile);  // the loads fly under the main loop
-
-      // ---- main loop: one wgmma group per k-block; the stage of k-block i - 1 is released once group i is issued ----
-      uint32_t prev_stage = 0;
-      for (int kb = 0; kb < kb_cnt; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-        const uint64_t da = make_smem_desc_sw128(sa + wg * (64 * 128), 16, 1024);
-        const uint64_t db = make_smem_desc_sw128(sa + BM * BK * 2, 16, 1024);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          // advance 16 elements (32 B) along K inside the 128-B swizzle row: +2 in the (addr >> 4) field
-          Wgmma<BN, kBf16>::ss(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
-        }
-        wgmma_commit();
-        if (kb > 0) {
-          wgmma_wait<1>();
-          if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-        }
-        prev_stage = stage;
-        if (++stage == Cfg::kStages) {
-          stage = 0;
-          phase ^= 1u;
-        }
-      }
-      wgmma_wait<0>();
-      reg_fence(acc);
-      if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-
-      // ---- rows of this thread; which group(s) of the per-branch vector they belong to ----
-      long long row[2];
-      bool row_ok[2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int r = rbase + 8 * h;
-        if (!g.conv) {
-          row[h] = static_cast<long long>(m_tile) * BM + r;
-          row_ok[h] = row[h] < M;
-        } else {
-          const int x = r % g.TW, y = (r / g.TW) % g.TH, n = r / (g.TW * g.TH);
-          row_ok[h] = (n < g.TN) && (x0 + x < g.W) && (y0 + y < g.H) && (n0 + n < g.NI);
-          row[h] = (static_cast<long long>(n0 + n) * g.H + (y0 + y)) * g.W + (x0 + x);
-        }
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");  // MMA warpgroups only: column constants visible
-
-      if (ep.partial) {
-        // split-K: raw fp32 accumulators of this K range -> partial[split][row][N]; the reduction kernel sums the
-        // splits in a fixed order and applies the whole epilogue (deterministic: no atomics)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (!row_ok[h]) continue;
-          float* prow = ep.partial + (static_cast<long long>(split) * M + row[h]) * N;
-#pragma unroll
-          for (int j = 0; j < BN / 8; ++j) {
-            const int col = n_tile * BN + 8 * j + q2;
-            if (col < N) *reinterpret_cast<float2*>(prow + col) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-          }
-        }
-        continue;
-      }
-
-      // one 32-column chunk: tile columns [32 c, 32 c + 32) of both rows -> staging buffer -> TMA store
-      auto stage_and_store = [&](uint8_t* obuf, int col0) {
-        fence_proxy_async_smem();
-        if (issuer) tma_store_wait_read0();  // see "Staging-buffer reuse" below
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (issuer) {
-          if (g.conv)
-            tma_store_4d(&tmOut, obuf, col0, x0, y0, n0);
-          else
-            tma_store_2d(&tmOut, obuf, col0, m_tile * BM);
-          tma_store_commit();
-        }
-      };
-
-      if (ep.act != MIMO_ACT_GEGLU) {
-        const float scale = ep.scale;
-        bool rv_uniform = false;
-        if (ep.rowvec) {
-          uint32_t gf, gl;
-          tile_groups(m_tile, gf, gl);
-          rv_uniform = gf == gl;
-        }
-        const bool need_rv = ep.rowvec != nullptr && !rv_uniform;  // uniform per tile
-        // mode 0: no column constants, unit scale, no residual -> accumulators are packed as they are;
-        //      1: y = acc * scale + consts (+ residual);  2: as 1, plus per-row vectors (tile straddles groups)
-        const int mode = (!kRes && !do_silu && !need_rv && ep.bias == nullptr && ep.rowvec == nullptr && scale == 1.0f)
-                             ? 0 : (need_rv ? 2 : 1);
-        const T* rv[2];
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-          rv[h] = (need_rv && row_ok[h])
-                      ? static_cast<const T*>(ep.rowvec) + static_cast<long long>(static_cast<uint32_t>(row[h]) / rpg) * ep.ld_rowvec
-                      : nullptr;
-#pragma unroll
-        for (int c = 0; c < NCHUNK; ++c) {
-          uint8_t* obuf = sOut + (oc & 1u) * kChunk;
-          ++oc;
-          const int col0 = n_tile * BN + c * 32;
-          [[maybe_unused]] uint32_t rslot = 0;
-          if constexpr (kRes) {
-            const uint32_t k = rc++;
-            rslot = k % Cfg::kResSlots;
-            mbar_wait(&res_full[rslot], (k / Cfg::kResSlots) & 1u);
-          }
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int j = 4 * c + jj;
-            const float2 cst0 = *reinterpret_cast<const float2*>(sb + c * 32 + 8 * jj + q2);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int r = rbase + 8 * h;
-              const int off = r * 64 + ((jj ^ sw[h]) << 4) + q2 * 2;
-              float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
-              if (mode != 0) {
-                float c0 = cst0.x, c1 = cst0.y;
-                // the per-row vector joins the column constants FIRST, as load_consts() pre-sums them when a tile lies
-                // inside one group
-                if (mode == 2 && rv[h] && col0 + 8 * jj + q2 < N) {
-                  const float2 t = C::unpack(__ldg(reinterpret_cast<const unsigned int*>(rv[h] + col0 + 8 * jj + q2)));
-                  c0 = fmaf(t.x, scale, c0);
-                  c1 = fmaf(t.y, scale, c1);
-                }
-                f0 = fmaf(f0, scale, c0);
-                f1 = fmaf(f1, scale, c1);
-              }
-              if constexpr (kRes) {
-                const float2 t = C::unpack(*reinterpret_cast<const uint32_t*>(sRes + rslot * kChunk + off));
-                f0 = fmaf(t.x, scale, f0);
-                f1 = fmaf(t.y, scale, f1);
-              }
-              if (do_silu) {
-                f0 = silu_f(f0);
-                f1 = silu_f(f1);
-              }
-              *reinterpret_cast<uint32_t*>(obuf + off) = C::pack(f0, f1);
-            }
-          }
-          if constexpr (kRes) {
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&res_empty[rslot]);
-          }
-          stage_and_store(obuf, col0);
-        }
-      } else {
-        // GEGLU: tile columns [0, BN/2) are values, [BN/2, BN) the matching gates (same thread, BN/16 fragments on)
-        constexpr int HALF = BN / 2;
-#pragma unroll
-        for (int c = 0; c < HALF / 32; ++c) {
-          uint8_t* obuf = sOut + (oc & 1u) * kChunk;
-          ++oc;
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int j = 4 * c + jj, jg = j + HALF / 8;
-            const float2 cv = *reinterpret_cast<const float2*>(sb + c * 32 + 8 * jj + q2);
-            const float2 cg = *reinterpret_cast<const float2*>(sb + HALF + c * 32 + 8 * jj + q2);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int r = rbase + 8 * h;
-              const float f0 = (acc[4 * j + 2 * h] + cv.x) * gelu_erf_fast(acc[4 * jg + 2 * h] + cg.x);
-              const float f1 = (acc[4 * j + 2 * h + 1] + cv.y) * gelu_erf_fast(acc[4 * jg + 2 * h + 1] + cg.y);
-              *reinterpret_cast<uint32_t*>(obuf + r * 64 + ((jj ^ sw[h]) << 4) + q2 * 2) = C::pack(f0, f1);
-            }
-          }
-          stage_and_store(obuf, n_tile * HALF + c * 32);
-        }
-      }
-    }
-    if (issuer) tma_store_wait_all();
-  }
+// e4m3 A [M, K] and W [N, K] with one fp32 scale per row of each, 16-bit output: GEMM rows only (g.conv == 0, tmA1 ==
+// tmA0 and never read, no split-K)
+template <int BN, bool kBf16, bool kRes>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_e4m3_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
+                 const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOut,
+                 const __grid_constant__ CUtensorMap tmRes, int M, int N, int num_m_tiles, int num_n_tiles,
+                 int num_k_blocks, ConvGeom g, EpiArgs ep, const float* __restrict__ a_scale,
+                 const float* __restrict__ w_scale) {
+  constexpr bool kE4m3 = true;
+#include "gemm_wgmma_body.cuh"
 }
 
 // Staging-buffer reuse: the two 8 KiB buffers alternate per chunk. The issuer executes cp.async.bulk.wait_group.read 0
@@ -578,6 +230,51 @@ static int launch_bn(int bn, bool res, const Maps& m, int M, int N, int mt, int 
                  : launch_cfg<256, kBf16, false>(m, M, N, mt, nt, nkb, g, ep, st);
   }
   return set_error(MIMO_ERR_ARG, "gemm: unsupported BN");
+}
+
+int pick_bn(int N, bool geglu, long long m_tiles);
+
+// ptxas (CUDA 12.9, -O3), per thread at the 168-register cap of 320 threads:
+//   gemm_e4m3_kernel<192, *, *>: 144-155 registers, no spills
+//   gemm_e4m3_kernel<256, f16 / bf16, no residual>: 168 registers, 32 / 16 B spill stores, 36 / 20 B spill loads
+//   gemm_e4m3_kernel<256, *, residual>: 168 registers, 32 B spill stores, 48 B spill loads
+//   (gemm_wgmma_kernel<256, *, *>, for comparison: 168 registers, 8 B spill stores, 8-16 B spill loads)
+// e4m3 tile widths (gemm_e4m3_kernel instantiations): 192 and 256 are the widths pick_bn gives the LN-fed GEMMs of the
+// UNet (q|k|v N = 3 C: 960 / 1920 -> 192, 3840 -> 256; GEGLU N = 8 C -> 256).
+template <bool kBf16>
+static int launch_e4m3(int bn, bool res, const Maps& m, int M, int N, int mt, int nt, int nkb, const ConvGeom& g,
+                       const EpiArgs& ep, const float* a_scale, const float* w_scale, cudaStream_t st) {
+  auto run = [&](auto kern, int smem) -> int {
+    static bool attr_done[2][2][2] = {};  // [bn == 256][kBf16][res]
+    bool& done = attr_done[bn == 256][kBf16][res];
+    if (!done) {
+      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+      if (e != cudaSuccess) return set_cuda_error("cudaFuncSetAttribute(gemm_e4m3)", e);
+      done = true;
+    }
+    const int tiles = mt * nt;
+    const int grid = tiles < num_sms() ? tiles : num_sms();
+    cudaError_t e = launch_k(kern, dim3(grid), dim3(kGemmThreads), smem, st, m.a0, m.a1, m.b, m.out, m.res, M, N, mt, nt,
+                             nkb, g, ep, a_scale, w_scale);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    if (e != cudaSuccess) return set_cuda_error("gemm_e4m3 launch", e);
+    return MIMO_OK;
+  };
+  if (bn == 192)
+    return res ? run(gemm_e4m3_kernel<192, kBf16, true>, GemmCfg<192, true, true>::kSmemBytes)
+               : run(gemm_e4m3_kernel<192, kBf16, false>, GemmCfg<192, false, true>::kSmemBytes);
+  if (bn == 256)
+    return res ? run(gemm_e4m3_kernel<256, kBf16, true>, GemmCfg<256, true, true>::kSmemBytes)
+               : run(gemm_e4m3_kernel<256, kBf16, false>, GemmCfg<256, false, true>::kSmemBytes);
+  return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3: unsupported BN");
+}
+
+// e4m3 tile width: pick_bn's rule over the instantiated widths {256, 192} - least padded columns, then the wider; GEGLU
+// takes pick_bn's own width (it fixes the weight packing, mimo_gemm_geglu_granule) and must be one of them.
+static int pick_bn_e4m3(int N, bool geglu) {
+  if (geglu) return pick_bn(N, true, 1 << 20);
+  const int pad256 = (N + 255) / 256 * 256 - N, pad192 = (N + 191) / 192 * 192 - N;
+  return pad192 < pad256 ? 192 : 256;
 }
 
 static int g_force_bn = 0;
@@ -731,6 +428,62 @@ extern "C" int mimo_gemm(const mimo_gemm_params* p, void* stream) {
                                        : launch_bn<false>(bn, res, m, p->M, p->N, mt, nt, nkb, g, ep, st);
   if (rc || splits == 1) return rc;
   return launch_reduce(p->dtype, ep.partial, splits, p->M, p->N, p->ep, p->out, p->ldo, st);
+}
+
+extern "C" int mimo_gemm_e4m3(const mimo_gemm_e4m3_params* p, void* stream) {
+  if (!p || !p->a || !p->w || !p->out || !p->a_scale || !p->w_scale)
+    return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3: null pointer");
+  if (p->M <= 0 || p->N <= 0 || p->K <= 0) return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3: empty problem");
+  if ((p->K % 16) || (p->lda % 16) || (p->ldw % 16))
+    return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3: K, lda, ldw must be multiples of 16");
+  if ((p->N % 8) || (p->ldo % 8)) return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3: N, ldo must be multiples of 8");
+  if ((reinterpret_cast<uintptr_t>(p->a) | reinterpret_cast<uintptr_t>(p->w) | reinterpret_cast<uintptr_t>(p->out) |
+       reinterpret_cast<uintptr_t>(p->ep.residual)) % 16)
+    return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3: a, w, out, residual must be 16-byte aligned");
+  if (p->ep.residual && (p->ep.ld_res % 8)) return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3: ld_res % 8 != 0");
+  if (p->workspace || p->workspace_bytes) return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3: split-K is not supported");
+  const bool geglu = p->ep.act == MIMO_ACT_GEGLU;
+  if (geglu && (p->ep.residual || p->ep.rowvec))
+    return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3: GEGLU takes neither a residual nor a row vector");
+  const int bn = pick_bn_e4m3(p->N, geglu);
+  if (geglu && (p->N % bn)) return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3: GEGLU needs N % tile == 0");
+  if (bn != 192 && bn != 256) return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3: GEGLU needs N % 256 == 0");
+  if (int rc = ensure_device()) return rc;
+  const int mt = (p->M + BM - 1) / BM;
+  const int nt = (p->N + bn - 1) / bn;
+  const int nkb = (p->K + 2 * BK - 1) / (2 * BK);
+  const bool res = p->ep.residual != nullptr && !geglu;
+
+  Maps m;
+  const uint64_t adim[2] = {static_cast<uint64_t>(p->K), static_cast<uint64_t>(p->M)};
+  const uint64_t astr[1] = {static_cast<uint64_t>(p->lda)};
+  const uint32_t abox[2] = {2 * BK, BM};
+  if (int rc = encode_tmap(&m.a0, kTmapU8, 2, p->a, adim, astr, abox)) return rc;
+  m.a1 = m.a0;
+  const uint64_t bdim[2] = {static_cast<uint64_t>(p->K), static_cast<uint64_t>(p->N)};
+  const uint64_t bstr[1] = {static_cast<uint64_t>(p->ldw)};
+  const uint32_t bbox[2] = {2 * BK, static_cast<uint32_t>(bn)};
+  if (int rc = encode_tmap(&m.b, kTmapU8, 2, p->w, bdim, bstr, bbox)) return rc;
+  const int n_out = geglu ? p->N / 2 : p->N;
+  const uint64_t odim[2] = {static_cast<uint64_t>(n_out), static_cast<uint64_t>(p->M)};
+  const uint64_t ostr[1] = {static_cast<uint64_t>(p->ldo) * 2};
+  const uint32_t obox[2] = {32, BM};
+  if (int rc = encode_tmap(&m.out, p->dtype, 2, p->out, odim, ostr, obox, 64)) return rc;
+  m.res = m.out;
+  if (res) {
+    const uint64_t rstr[1] = {static_cast<uint64_t>(p->ep.ld_res) * 2};
+    if (int rc = encode_tmap(&m.res, p->dtype, 2, p->ep.residual, odim, rstr, obox, 64)) return rc;
+  }
+  ConvGeom g = {};
+  g.kb0 = nkb;
+  g.c0 = p->K;
+  g.chunk_bytes = kChunk;
+  g.splits = 1;
+  g.kb_split = nkb;
+  const EpiArgs ep = make_epi(p->ep, p->N);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return p->dtype == MIMO_BF16 ? launch_e4m3<true>(bn, res, m, p->M, p->N, mt, nt, nkb, g, ep, p->a_scale, p->w_scale, st)
+                               : launch_e4m3<false>(bn, res, m, p->M, p->N, mt, nt, nkb, g, ep, p->a_scale, p->w_scale, st);
 }
 
 // One implicit-GEMM convolution launch: `ntaps` taps at offsets (tdx, tdy) over the [n, h, w, c] input(s); the output

@@ -551,6 +551,115 @@ static void launch_ln5(int L, const void* x, const void* gamma, const void* beta
     launch_k(layernorm5_kernel<kBf16, 32>, dim3(blocks), dim3(256), 0, st, x, gamma, beta, out, rows, eps, pe, rpf, frames, pe_off);
 }
 
+// ------------------------------------------------------------------------------------------------
+// LayerNorm (+ PE) -> e4m3 rows with one fp32 scale each (the A operand of mimo_gemm_e4m3)
+// ------------------------------------------------------------------------------------------------
+// L lanes per row, NV 8-channel vectors per lane (C = 320 / 640 / 1280: L = 8 / 16 / 32 and NV = 5, every lane busy; any
+// other C: L = 32, NV = 8, predicated). The row's fp32 values stay in registers between the amax and the conversion.
+template <bool kBf16, int L, int NV>
+__global__ void __launch_bounds__(256)
+layernorm_e4m3_kernel(const void* __restrict__ x, const void* __restrict__ gamma, const void* __restrict__ beta,
+                      uint8_t* __restrict__ out, float* __restrict__ scale, long long rows, int Cdim, float eps,
+                      const void* __restrict__ pe, long long rows_per_frame, int frames, int pe_off) {
+  using C = Cvt<kBf16>;
+  using T = typename C::T;
+  constexpr int R = 32 / L;  // rows per warp
+  pdl_launch_dependents();
+  pdl_wait();
+  const int lane = threadIdx.x & 31;
+  const int sub = lane % L;
+  const long long row = (static_cast<long long>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5)) * R + lane / L;
+  const bool ok = row < rows;  // no early exit: the lanes of a warp shuffle together
+  const int vecs = Cdim >> 3;
+  const T* xr = static_cast<const T*>(x) + (ok ? row : 0) * Cdim;
+  uint4 u[NV];
+  float sum = 0.f;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const int v = sub + i * L;
+    u[i] = (ok && v < vecs) ? *reinterpret_cast<const uint4*>(xr + v * 8) : make_uint4(0, 0, 0, 0);
+    const uint32_t w[4] = {u[i].x, u[i].y, u[i].z, u[i].w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 t = C::unpack(w[j]);
+      sum += t.x + t.y;
+    }
+  }
+#pragma unroll
+  for (int o = L / 2; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  const float mean = sum / static_cast<float>(Cdim);
+  float sq = 0.f;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    if (sub + i * L < vecs) {
+      const uint32_t w[4] = {u[i].x, u[i].y, u[i].z, u[i].w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 t = C::unpack(w[j]);
+        const float d0 = t.x - mean, d1 = t.y - mean;
+        sq += d0 * d0 + d1 * d1;
+      }
+    }
+  }
+#pragma unroll
+  for (int o = L / 2; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
+  const float rstd = rsqrtf(sq / static_cast<float>(Cdim) + eps);
+  const T* per = (pe && ok) ? static_cast<const T*>(pe) + (pe_off + (row / rows_per_frame) % frames) * Cdim : nullptr;
+  float y[NV][8];
+  float amax = 0.f;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const int v = sub + i * L;
+    if (v < vecs) {
+      const uint4 ug = __ldg(reinterpret_cast<const uint4*>(static_cast<const T*>(gamma) + v * 8));
+      const uint4 ub = __ldg(reinterpret_cast<const uint4*>(static_cast<const T*>(beta) + v * 8));
+      const uint4 up = per ? __ldg(reinterpret_cast<const uint4*>(per + v * 8)) : make_uint4(0, 0, 0, 0);
+      const uint32_t w[4] = {u[i].x, u[i].y, u[i].z, u[i].w};
+      const uint32_t wg[4] = {ug.x, ug.y, ug.z, ug.w};
+      const uint32_t wb[4] = {ub.x, ub.y, ub.z, ub.w};
+      const uint32_t wp[4] = {up.x, up.y, up.z, up.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 t = C::unpack(w[j]);
+        const float2 g2 = C::unpack(wg[j]);
+        const float2 b2 = C::unpack(wb[j]);
+        float y0 = (t.x - mean) * rstd * g2.x + b2.x;
+        float y1 = (t.y - mean) * rstd * g2.y + b2.y;
+        if (per) {
+          // as mimo_layernorm: LN's output is rounded to the storage type before the encoding is added
+          const float2 p2 = C::unpack(wp[j]);
+          y0 = C::to_f(C::from_f(y0)) + p2.x;
+          y1 = C::to_f(C::from_f(y1)) + p2.y;
+        }
+        y[i][2 * j] = y0;
+        y[i][2 * j + 1] = y1;
+        amax = fmaxf(amax, fmaxf(fabsf(y0), fabsf(y1)));
+      }
+    }
+  }
+#pragma unroll
+  for (int o = L / 2; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  if (!ok) return;
+  const float inv = amax == 0.f ? 1.f : 448.0f / amax;
+  if (sub == 0) scale[row] = amax == 0.f ? 1.f : amax / 448.0f;
+  uint8_t* orow = out + row * Cdim;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const int v = sub + i * L;
+    if (v < vecs) {
+      uint32_t q[2];  // 8 bytes: elements 4 j .. 4 j + 3 in q[j], lowest address in the lowest byte
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        uint16_t lo, hi;  // cvt packs its first source into the upper byte
+        asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(lo) : "f"(y[i][4 * j + 1] * inv), "f"(y[i][4 * j] * inv));
+        asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(hi) : "f"(y[i][4 * j + 3] * inv), "f"(y[i][4 * j + 2] * inv));
+        q[j] = static_cast<uint32_t>(lo) | (static_cast<uint32_t>(hi) << 16);
+      }
+      *reinterpret_cast<uint2*>(orow + v * 8) = make_uint2(q[0], q[1]);
+    }
+  }
+}
+
 }  // namespace mimo
 
 using namespace mimo;
@@ -772,5 +881,39 @@ extern "C" int mimo_layernorm(const void* x, const void* gamma, const void* beta
              static_cast<long long>(rows_per_frame), frames, pe_frame_offset);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_cuda_error("layernorm launch", e);
+  return MIMO_OK;
+}
+
+extern "C" int mimo_layernorm_e4m3(const void* x, const void* gamma, const void* beta, void* out, float* scale,
+                                   int64_t rows, int32_t c, float eps, const void* pe, int64_t rows_per_frame,
+                                   int32_t frames, int32_t pe_frame_offset, int32_t dtype, void* stream) {
+  if (!x || !gamma || !beta || !out || !scale) return set_error(MIMO_ERR_ARG, "mimo_layernorm_e4m3: null pointer");
+  if (rows <= 0 || c <= 0 || (c % 16) || c > 32 * 8 * kLnMaxVec)
+    return set_error(MIMO_ERR_ARG, "mimo_layernorm_e4m3: c must be a multiple of 16 and <= 2048");
+  if (pe && (rows_per_frame <= 0 || frames <= 0)) return set_error(MIMO_ERR_ARG, "mimo_layernorm_e4m3: bad pe args");
+  if (int rc = ensure_device()) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int L = c == 320 ? 8 : (c == 640 ? 16 : (c == 1280 ? 32 : 0));
+  const unsigned blocks = div_up(rows, 8LL * (L ? 32 / L : 1));
+  uint8_t* o = static_cast<uint8_t*>(out);
+  const long long r = rows, rpf = pe ? rows_per_frame : 1;
+  cudaError_t e;
+#define MIMO_LN_E4M3(BF, LL, NV)                                                                                       \
+  e = launch_k(layernorm_e4m3_kernel<BF, LL, NV>, dim3(blocks), dim3(256), 0, st, x, gamma, beta, o, scale, r, c, eps, pe, \
+               rpf, frames, pe_frame_offset)
+  if (dtype == MIMO_BF16) {
+    if (L == 8) MIMO_LN_E4M3(true, 8, 5);
+    else if (L == 16) MIMO_LN_E4M3(true, 16, 5);
+    else if (L == 32) MIMO_LN_E4M3(true, 32, 5);
+    else MIMO_LN_E4M3(true, 32, kLnMaxVec);
+  } else {
+    if (L == 8) MIMO_LN_E4M3(false, 8, 5);
+    else if (L == 16) MIMO_LN_E4M3(false, 16, 5);
+    else if (L == 32) MIMO_LN_E4M3(false, 32, 5);
+    else MIMO_LN_E4M3(false, 32, kLnMaxVec);
+  }
+#undef MIMO_LN_E4M3
+  if (e == cudaSuccess) e = cudaGetLastError();
+  if (e != cudaSuccess) return set_cuda_error("layernorm_e4m3 launch", e);
   return MIMO_OK;
 }

@@ -19,6 +19,7 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass, field
+from pathlib import Path
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
@@ -129,6 +130,10 @@ class UNetEngine:
         self._graphs: Dict[tuple, dict] = {}
         self.use_graphs = True
         self._launches_per_forward = 0
+        # FP8 (set_fp8): e4m3 copies of the LN-fed projection weights, packed on first use; the fp16 / bf16 packs stay
+        self.fp8 = False
+        self.w8: Optional[Dict[str, dict]] = None
+        self._cache8: Optional[Path] = None  # file of the e4m3 copies in the weight cache (when one is set)
         # packed weights: from the on-disk cache when MIMO_B200_WEIGHT_CACHE is set and holds this state dict
         from .host import weight_cache as WC
         cache = WC.cache_dir()
@@ -136,6 +141,8 @@ class UNetEngine:
         if cache is not None:
             key = WC.fingerprint(sd, f"unet|{spec}|{dtype}|{L.load().mimo_version().decode()}")
             cfile = cache / f"unet-{key}.safetensors"
+            # the e4m3 copies are a function of the packed weights, which `key` already identifies: no second pass over sd
+            self._cache8 = cache / f"unet-e4m3-{WC.fingerprint({}, extra=f'unet-e4m3|{key}')}.safetensors"
             if cfile.exists():
                 st = WC.load(cfile, self.device)
                 self.w, self.resnets, self.xf_paths = st["w"], st["resnets"], st["xf_paths"]
@@ -239,6 +246,45 @@ class UNetEngine:
             bs.append(b)
         W["temb_all"] = (torch.cat(ws, 0).contiguous(), torch.cat(bs, 0).contiguous())
 
+    def _pack_e4m3(self) -> Dict[str, dict]:
+        """e4m3 copies (one fp32 scale per output channel, ops.pack_e4m3_weight) of the projections that read a LayerNorm
+        output: each spatial transformer's q|k|v and GEGLU, each motion module's two q|k|v and its GEGLU. The GEGLU copy is
+        quantized from the tile-interleaved pack, so its scales come in the same order."""
+        q = ops.pack_e4m3_weight
+        w8: Dict[str, dict] = {}
+        for p in self.xf_paths:
+            w8[p] = {"qkv": q(self.w[p]["qkv"]), "geglu": q(self.w[p]["geglu"][0])}
+        for p, m in self.w.items():
+            if isinstance(m, dict) and "attn" in m:
+                w8[p] = {"qkv": [q(a["qkv"]) for a in m["attn"]], "geglu": q(m["geglu"][0])}
+        return w8
+
+    def set_fp8(self, on: bool) -> None:
+        """Run the LN-fed projections (see _pack_e4m3) as LayerNorm -> e4m3 rows + scales -> e4m3 GEMM. Captured graphs
+        are dropped whenever the setting changes."""
+        on = bool(on)
+        if on == self.fp8:
+            return
+        if on and self.w8 is None:
+            from .host import weight_cache as WC
+            cfile = self._cache8
+            if cfile is not None and cfile.exists():
+                self.w8 = WC.load(cfile, self.device)
+            else:
+                self.w8 = self._pack_e4m3()
+                if cfile is not None:
+                    WC.save(cfile, self.w8)
+        self.fp8 = on
+        self._graphs.clear()
+
+    def fp8_bytes(self) -> int:
+        """device bytes of the e4m3 copies (0 before the first set_fp8(True))"""
+        out = 0
+        for m in (self.w8 or {}).values():
+            for wq, ws in [m["geglu"]] + (m["qkv"] if isinstance(m["qkv"], list) else [m["qkv"]]):
+                out += wq.numel() * wq.element_size() + ws.numel() * ws.element_size()
+        return out
+
     # ------------------------------------------------------------------------------------------------
     def _sinusoid(self, timesteps: torch.Tensor) -> torch.Tensor:
         """Timesteps(flip_sin_to_cos, shift 0) in fp32, cast to the model dtype (unet_3d_edit_bkfill.py:462-467)."""
@@ -304,9 +350,13 @@ class UNetEngine:
             res = x0
         return ops.conv3x3(t, r["c2"][0], n, h, w, bias=r["c2"][1], residual=res)
 
-    def _ff(self, x, ln, geglu, ffo):
-        nh = ops.layernorm(x, *ln)
-        gg = ops.gemm(nh, geglu[0], bias=geglu[1], act=L.ACT_GEGLU)
+    def _ff(self, x, ln, geglu, ffo, geglu8=None):
+        if geglu8 is None:
+            nh = ops.layernorm(x, *ln)
+            gg = ops.gemm(nh, geglu[0], bias=geglu[1], act=L.ACT_GEGLU)
+        else:
+            q, sc = ops.layernorm_e4m3(x, *ln)
+            gg = ops.gemm_e4m3(q, sc, *geglu8, x.dtype, bias=geglu[1], act=L.ACT_GEGLU)
         return ops.gemm(gg, ffo[0], bias=ffo[1], residual=x)
 
     def _xf_read(self, p, x, n, hw, rows_per_branch, st):
@@ -314,8 +364,13 @@ class UNetEngine:
         C = m["C"]
         hcur = ops.groupnorm(x, *m["gn"], n, hw, groups=self.spec.norm_num_groups, eps=1e-6)
         hcur = ops.gemm(hcur, m["pin"][0], bias=m["pin"][1])
-        nh = ops.layernorm(hcur, *m["ln1"])
-        qkv = ops.gemm(nh, m["qkv"])
+        w8 = self.w8[p] if self.fp8 else None
+        if w8 is None:
+            nh = ops.layernorm(hcur, *m["ln1"])
+            qkv = ops.gemm(nh, m["qkv"])
+        else:
+            q, sc = ops.layernorm_e4m3(hcur, *m["ln1"])
+            qkv = ops.gemm_e4m3(q, sc, *w8["qkv"], hcur.dtype)
         bank = st["banks"].get(p)
         if bank is not None:
             att = ops.attn_spatial(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], n, hw, self.spec.heads,
@@ -325,7 +380,7 @@ class UNetEngine:
             att = ops.attn_spatial(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], n, hw, self.spec.heads)
         hcur = ops.gemm(att, m["o1"][0], bias=m["o1"][1], residual=hcur, rowvec=st["xattn"][p],
                         rows_per_group=rows_per_branch)
-        hcur = self._ff(hcur, m["ln3"], m["geglu"], m["ffo"])
+        hcur = self._ff(hcur, m["ln3"], m["geglu"], m["ffo"], w8["geglu"] if w8 else None)
         return ops.gemm(hcur, m["pout"][0], bias=m["pout"][1], residual=x)
 
     def _motion(self, p, x, b, f, hw):
@@ -353,12 +408,17 @@ class UNetEngine:
             hw_l = hw // G
             ops.gemm(hcur, m["pin"][0], out=xg.bufs["A"].view(n * hw, C, x.dtype), bias=m["pin"][1])
             hcur = xg.pull(0, "A", torch.empty((b * F_ * hw_l, C), dtype=x.dtype, device=x.device), b, f, hw, C)
-        for a in m["attn"]:
-            nh = ops.layernorm(hcur, *a["ln"], pe=a["pe"], rows_per_frame=hw_l, frames=F_)
-            qkv = ops.gemm(nh, a["qkv"])
+        w8 = self.w8[p] if self.fp8 else None
+        for i, a in enumerate(m["attn"]):
+            if w8 is None:
+                nh = ops.layernorm(hcur, *a["ln"], pe=a["pe"], rows_per_frame=hw_l, frames=F_)
+                qkv = ops.gemm(nh, a["qkv"])
+            else:  # LN + PE run on this GPU's tokens after the exchange, so FP8 needs no extra communication
+                q, sc = ops.layernorm_e4m3(hcur, *a["ln"], pe=a["pe"], rows_per_frame=hw_l, frames=F_)
+                qkv = ops.gemm_e4m3(q, sc, *w8["qkv"][i], hcur.dtype)
             att = ops.attn_temporal(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], b, F_, hw_l, self.spec.heads)
             hcur = ops.gemm(att, a["o"][0], bias=a["o"][1], residual=hcur)
-        hcur = self._ff(hcur, m["ffn"], m["geglu"], m["ffo"])
+        hcur = self._ff(hcur, m["ffn"], m["geglu"], m["ffo"], w8["geglu"] if w8 else None)
         if G == 1:
             return ops.gemm(hcur, m["pout"][0], bias=m["pout"][1], residual=x)
         ops.gemm(hcur, m["pout"][0], out=xg.bufs["B"].view(b * F_ * hw_l, C, x.dtype), bias=m["pout"][1])

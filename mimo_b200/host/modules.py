@@ -270,6 +270,35 @@ class UNet3DConditionModel(_UNetBase):
                         motion_max_len=self._motion_max_len)
         self._spec.inflated_groupnorm = self.use_inflated_groupnorm
 
+    _fp8 = False
+
+    def enable_fp8(self):
+        """Run the q|k|v and GEGLU projections that read a LayerNorm output in FP8 (e4m3 activations with one scale per
+        token, e4m3 weights with one scale per output channel, fp32 accumulation). Everything else stays in the model
+        dtype. The e4m3 weight copies are made on first use and kept; captured CUDA graphs of the forward are dropped."""
+        if self.dtype not in (torch.float16, torch.bfloat16):
+            raise MimoError(f"enable_fp8() needs an fp16 or bf16 model, not {self.dtype}")
+        self._fp8 = True
+        if self._engine is not None:
+            self._engine.set_fp8(True)
+        return self
+
+    def disable_fp8(self):
+        """Back to the model dtype for every projection (the e4m3 copies stay packed for a later enable_fp8())."""
+        self._fp8 = False
+        if self._engine is not None:
+            self._engine.set_fp8(False)
+        return self
+
+    @property
+    def fp8_enabled(self) -> bool:
+        return self._fp8
+
+    def engine(self) -> E.UNetEngine:
+        eng = super().engine()
+        eng.set_fp8(self._fp8)
+        return eng
+
     @classmethod
     def from_pretrained_2d(cls, pretrained_model_path, motion_module_path, subfolder=None,
                            unet_additional_kwargs=None, mm_zero_proj_out=False):

@@ -46,6 +46,18 @@ class GemmParams(C.Structure):
     ]
 
 
+class GemmE4m3Params(C.Structure):
+    _fields_ = [
+        ("a", C.c_void_p), ("lda", C.c_int64), ("a_scale", C.c_void_p),
+        ("w", C.c_void_p), ("ldw", C.c_int64), ("w_scale", C.c_void_p),
+        ("out", C.c_void_p), ("ldo", C.c_int64),
+        ("M", C.c_int32), ("N", C.c_int32), ("K", C.c_int32),
+        ("dtype", C.c_int32),
+        ("ep", Epilogue),
+        ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64),
+    ]
+
+
 class Conv3x3Params(C.Structure):
     _fields_ = [
         ("x0", C.c_void_p), ("c0", C.c_int32),
@@ -148,6 +160,7 @@ SYMBOLS = {
     "mimo_abi_sizeof": (C.c_int, [C.c_int]),
     "mimo_gemm": (C.c_int, [C.POINTER(GemmParams), _VP]),
     "mimo_gemm_geglu_granule": (C.c_int, [_I32]),
+    "mimo_gemm_e4m3": (C.c_int, [C.POINTER(GemmE4m3Params), _VP]),
     "mimo_conv3x3": (C.c_int, [C.POINTER(Conv3x3Params), _VP]),
     "mimo_conv_up2x": (C.c_int, [C.POINTER(Conv3x3Params), _VP]),
     "mimo_im2col3x3": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I64, _I32, _VP]),
@@ -158,6 +171,7 @@ SYMBOLS = {
     "mimo_groupnorm_window_apply": (C.c_int, [C.POINTER(GroupNormWindowParams), _VP]),
     "mimo_groupnorm_window_table_bytes": (C.c_int64, [C.POINTER(GroupNormWindowParams)]),
     "mimo_layernorm": (C.c_int, [_VP, _VP, _VP, _VP, _I64, _I32, _F, _VP, _I64, _I32, _I32, _I32, _VP]),
+    "mimo_layernorm_e4m3": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _I64, _I32, _F, _VP, _I64, _I32, _I32, _I32, _VP]),
     "mimo_attn_spatial": (C.c_int, [C.POINTER(AttnParams), _VP]),
     "mimo_attn_temporal": (C.c_int, [C.POINTER(AttnTemporalParams), _VP]),
     "mimo_exchange": (C.c_int, [C.POINTER(ExchangeParams), _VP]),
@@ -202,7 +216,7 @@ def load() -> C.CDLL:
         fn.restype = res
         fn.argtypes = args
     for which, st in enumerate((Epilogue, GemmParams, Conv3x3Params, GroupNormParams, AttnParams, AttnTemporalParams,
-                             ExchangeParams, CfgMultistepParams, GroupNormWindowParams)):
+                             ExchangeParams, CfgMultistepParams, GroupNormWindowParams, GemmE4m3Params)):
         if lib.mimo_abi_sizeof(which) != C.sizeof(st):
             raise MimoError(f"ABI mismatch: {st.__name__} is {C.sizeof(st)} bytes in lib.py but "
                             f"{lib.mimo_abi_sizeof(which)} in {LIB_PATH.name}; rebuild the library")

@@ -128,6 +128,33 @@ def gemm(a: torch.Tensor, w: torch.Tensor, out: Optional[torch.Tensor] = None, *
     return out
 
 
+def gemm_e4m3(a: torch.Tensor, a_scale: torch.Tensor, w: torch.Tensor, w_scale: torch.Tensor, dtype: torch.dtype,
+              out: Optional[torch.Tensor] = None, *, bias=None, rowvec=None, rows_per_group=1, residual=None, scale=1.0,
+              act=L.ACT_NONE) -> torch.Tensor:
+    """out[M, N(or N/2 for GEGLU)] = epilogue((a[M, K] @ w[N, K]^T) * a_scale[:, None] * w_scale[None, :]): a and w are
+    torch.float8_e4m3fn, the scales fp32, out / bias / residual `dtype`."""
+    assert a.dtype == torch.float8_e4m3fn and w.dtype == torch.float8_e4m3fn
+    assert a.dim() == 2 and w.dim() == 2 and a.shape[1] == w.shape[1] and a.stride(1) == 1 and w.stride(1) == 1
+    assert a_scale.dtype == torch.float32 and w_scale.dtype == torch.float32
+    assert a_scale.shape == (a.shape[0],) and w_scale.shape == (w.shape[0],)
+    M, K = a.shape
+    N = w.shape[0]
+    n_out = N // 2 if act == L.ACT_GEGLU else N
+    if out is None:
+        out = torch.empty((M, n_out), dtype=dtype, device=a.device)
+    assert out.shape == (M, n_out) and out.stride(1) == 1 and out.dtype == dtype
+    p = L.GemmE4m3Params()
+    p.a, p.lda, p.a_scale = _ptr(a), a.stride(0), _ptr(a_scale)
+    p.w, p.ldw, p.w_scale = _ptr(w), w.stride(0), _ptr(w_scale)
+    p.out, p.ldo = _ptr(out), out.stride(0)
+    p.M, p.N, p.K = M, N, K
+    p.dtype = _dt(out)
+    p.ep = _epilogue(bias, rowvec, rows_per_group, residual, scale, act)
+    with _Call("gemm_e4m3", 1, 2.0 * M * N * K, M * K + N * K + 4.0 * (M + N) + 2.0 * (M * n_out + (M * N if residual is not None else 0))):
+        L.check(L.load().mimo_gemm_e4m3(C.byref(p), _stream()), "mimo_gemm_e4m3")
+    return out
+
+
 def conv3x3(x0: torch.Tensor, w: torch.Tensor, n: int, h: int, wd: int, out: Optional[torch.Tensor] = None, *,
             x1: Optional[torch.Tensor] = None, bias=None, rowvec=None, rows_per_group: Optional[int] = None,
             residual=None, scale=1.0, act=L.ACT_NONE) -> torch.Tensor:
@@ -311,6 +338,20 @@ def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, *, eps=1
                                         _ptr(pe), int(rows_per_frame), int(frames), int(pe_frame_offset), _dt(x),
                                         _stream()), "mimo_layernorm")
     return out
+
+
+def layernorm_e4m3(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, *, eps=1e-5,
+                   pe: Optional[torch.Tensor] = None, rows_per_frame=1, frames=1, pe_frame_offset=0):
+    """layernorm() quantized per row for gemm_e4m3: returns (q [rows, C] float8_e4m3fn, scale [rows] fp32), with
+    q * scale ~ the fp32 LN(+PE) output (include/mimo_b200.h gives the exact rule)."""
+    assert x.is_contiguous() and x.dim() == 2
+    out = torch.empty(x.shape, dtype=torch.float8_e4m3fn, device=x.device)
+    sc = torch.empty((x.shape[0],), dtype=torch.float32, device=x.device)
+    with _Call("layernorm_e4m3", 1, 0.0, 2.0 * x.numel() + x.numel() + 4.0 * x.shape[0]):
+        L.check(L.load().mimo_layernorm_e4m3(_ptr(x), _ptr(gamma), _ptr(beta), _ptr(out), _ptr(sc), x.shape[0], x.shape[1],
+                                             float(eps), _ptr(pe), int(rows_per_frame), int(frames), int(pe_frame_offset),
+                                             _dt(x), _stream()), "mimo_layernorm_e4m3")
+    return out, sc
 
 
 def attn_spatial(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, n: int, lq: int, heads: int, *,
@@ -607,3 +648,26 @@ def pack_geglu_weight(w: torch.Tensor, b: Optional[torch.Tensor]):
         bv, bg = b[:inner].reshape(inner // g, g), b[inner:].reshape(inner // g, g)
         bp = torch.stack([bv, bg], dim=1).reshape(n2).contiguous()
     return wp, bp
+
+
+E4M3_MAX = 448.0
+
+
+def quantize_e4m3_rows(y: torch.Tensor):
+    """The per-row e4m3 rule of mimo_layernorm_e4m3 on the host: amax = max |y| of each row (in fp32), q = y * (448 /
+    amax) rounded to nearest and saturated, scale = amax / 448; a zero row gets scale 1. Returns (q float8_e4m3fn, scale
+    fp32). torch's cast does not saturate (it gives NaN past 448), hence the clamp. Both divisions are tensor / tensor:
+    torch turns a division by a Python scalar into a multiplication by its reciprocal, which is not the IEEE quotient."""
+    y = y.float()
+    amax = y.abs().amax(dim=1)
+    zero = amax == 0
+    inv = torch.where(zero, torch.ones_like(amax), torch.full_like(amax, E4M3_MAX) / amax)
+    scale = torch.where(zero, torch.ones_like(amax), amax / torch.full_like(amax, E4M3_MAX))
+    q = torch.clamp(y * inv[:, None], -E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn)
+    return q.contiguous(), scale.contiguous()
+
+
+def pack_e4m3_weight(w: torch.Tensor):
+    """A [N, K] weight (already in gemm's row order, e.g. pack_geglu_weight's) as (e4m3 [N, K], fp32 scale [N]): one
+    scale per output channel by quantize_e4m3_rows, so the rows' order - and the GEGLU tile interleave - is kept."""
+    return quantize_e4m3_rows(w)
