@@ -268,7 +268,8 @@ extern "C" int mimo_attn_temporal(const mimo_attn_temporal_params* p, void* stre
   if (p->batch <= 0 || p->q_frames <= 0 || p->kv_frames <= 0 || p->kv_frames > 32 || p->q_frames > 32 || p->hw <= 0 ||
       p->heads <= 0 || p->heads > 32 || p->d <= 0 || (p->d % 8) || p->d > 256 || (p->ld_q % 8) || (p->ld_kv % 8) || (p->ld_out % 8) ||
       (p->kv_frames % fpc))
-    return set_error(MIMO_ERR_ARG, "mimo_attn_temporal: need frames <= 32, heads <= 32, d % 8 == 0, kv_frames % chunk == 0");
+    return set_error(MIMO_ERR_ARG,
+                     "mimo_attn_temporal: need frames <= 32, heads <= 32, d % 8 == 0, d <= 256, kv_frames % chunk == 0");
   if (int rc = ensure_device()) return rc;
   TemporalArgs a;
   a.q = p->q;
@@ -291,6 +292,9 @@ extern "C" int mimo_attn_temporal(const mimo_attn_temporal_params* p, void* stre
   int hg = p->heads;
   auto smem_for = [&](int h) { return static_cast<size_t>(3) * 32 * (h * a.dpad + 8) * 2; };
   while (hg > 1 && (hg % 2 == 0) && smem_for(hg) > 100 * 1024) hg /= 2;
+  // the staging loop gives each lane 4 of a row's 16-byte vectors: hg * d / 8 <= 128. An odd head count that the loop
+  // above cannot halve (5 heads of 224) would leave vectors unstaged; one head per CTA always fits (d <= 256).
+  if (hg * (p->d / 8) > 128) hg = 1;
   if (smem_for(hg) > 227 * 1024) return set_error(MIMO_ERR_ARG, "mimo_attn_temporal: head dim too large");
   a.hg = hg;
   a.pitch = hg * a.dpad + 8;

@@ -26,6 +26,7 @@ import torch
 
 from . import lib as L
 from . import ops
+from .host.schema import MotionLayout
 
 SD = Dict[str, torch.Tensor]
 
@@ -47,6 +48,12 @@ class UNetSpec:
     # torch.nn.GroupNorm over all frames of the window (resnet.py:155-163, 185-192; unet_3d_edit_bkfill.py:236-247).
     # The packed weights do not depend on it, so it stays out of the repr that keys the weight cache.
     inflated_groupnorm: bool = field(default=True, repr=False)
+    # which blocks have motion modules and what each holds (only read when motion is True)
+    motion_layout: MotionLayout = MotionLayout()
+
+    def has_motion(self, block: str) -> bool:
+        """whether `block` ("down_blocks.i", "mid_block", "up_blocks.i") runs motion modules after its layers"""
+        return self.motion and self.motion_layout.placed(block, len(self.block_out_channels))
 
 
 def _dev(sd: SD, key: str, device, dtype) -> torch.Tensor:
@@ -123,6 +130,15 @@ class UNetEngine:
     """Executes the denoising UNet3D (motion=True) or the reference UNet2D bank pass (motion=False)."""
 
     def __init__(self, sd: SD, spec: UNetSpec, device, dtype=torch.float16):
+        if spec.motion:
+            bad = {c: d for c, d in spec.motion_layout.head_widths(spec.block_out_channels).items()
+                   if d != int(d) or d % 8 or d > 256}
+            if bad:
+                raise NotImplementedError(
+                    f"num_attention_heads={spec.motion_layout.heads}: the motion modules of widths "
+                    f"{', '.join(str(c) for c in sorted(bad))} get heads of "
+                    f"{', '.join(f'{bad[c]:g}' for c in sorted(bad))} channels; mimo_attn_temporal runs heads of a "
+                    "multiple of 8 channels, at most 256")
         L.check(L.load().mimo_device_check(torch.device(device).index or 0), "mimo_device_check")
         self.spec, self.device, self.dtype = spec, torch.device(device), dtype
         self.clip_state: Optional[dict] = None
@@ -190,18 +206,25 @@ class UNetEngine:
                 "geglu": pk.geglu(b + ".ff.net.0.proj"), "ffo": pk.lin(b + ".ff.net.2"),
             }
 
+        lay = spec.motion_layout
+
         def add_mm(p):
             t = p + ".temporal_transformer"
-            b = t + ".transformer_blocks.0"
-            m = {"gn": pk.norm(t + ".norm"), "pin": pk.lin(t + ".proj_in"), "pout": pk.lin(t + ".proj_out"),
-                 "ffn": pk.norm(b + ".ff_norm"), "geglu": pk.geglu(b + ".ff.net.0.proj"), "ffo": pk.lin(b + ".ff.net.2"),
-                 "attn": []}
-            for i in range(2):
-                a = f"{b}.attention_blocks.{i}"
-                qkv = torch.cat([pk.t(f"{a}.to_{x}.weight") for x in "qkv"], 0).contiguous()
-                pe = pk.t(a + ".pos_encoder.pe")[0].contiguous()  # [max_len, C]
-                m["attn"].append({"ln": pk.norm(f"{b}.norms.{i}"), "qkv": qkv, "o": pk.lin(a + ".to_out.0"), "pe": pe})
-            W[p] = m
+            blocks = []
+            for k in range(lay.blocks):
+                b = f"{t}.transformer_blocks.{k}"
+                blk = {"ffn": pk.norm(b + ".ff_norm"), "geglu": pk.geglu(b + ".ff.net.0.proj"),
+                       "ffo": pk.lin(b + ".ff.net.2"), "attn": []}
+                for i in range(lay.attn_blocks):
+                    a = f"{b}.attention_blocks.{i}"
+                    qkv = torch.cat([pk.t(f"{a}.to_{x}.weight") for x in "qkv"], 0).contiguous()
+                    att = {"ln": pk.norm(f"{b}.norms.{i}"), "qkv": qkv, "o": pk.lin(a + ".to_out.0")}
+                    if lay.pe:
+                        att["pe"] = pk.t(a + ".pos_encoder.pe")[0].contiguous()  # [max_len, C]
+                    blk["attn"].append(att)
+                blocks.append(blk)
+            W[p] = {"gn": pk.norm(t + ".norm"), "pin": pk.lin(t + ".proj_in"), "pout": pk.lin(t + ".proj_out"),
+                    "blocks": blocks}
 
         self.xf_paths: List[str] = []
         for i in range(nb):
@@ -210,14 +233,14 @@ class UNetEngine:
                 if i < nb - 1:
                     add_xf(f"down_blocks.{i}.attentions.{j}")
                     self.xf_paths.append(f"down_blocks.{i}.attentions.{j}")
-                if spec.motion:
+                if spec.has_motion(f"down_blocks.{i}"):
                     add_mm(f"down_blocks.{i}.motion_modules.{j}")
             if i < nb - 1:
                 W[f"down_blocks.{i}.down"] = pk.conv3(f"down_blocks.{i}.downsamplers.0.conv")
         add_resnet("mid_block.resnets.0")
         add_xf("mid_block.attentions.0")
         self.xf_paths.append("mid_block.attentions.0")
-        if spec.motion:
+        if spec.has_motion("mid_block"):
             add_mm("mid_block.motion_modules.0")
         add_resnet("mid_block.resnets.1")
         for i in range(nb):
@@ -226,7 +249,7 @@ class UNetEngine:
                 if i > 0:
                     add_xf(f"up_blocks.{i}.attentions.{j}")
                     self.xf_paths.append(f"up_blocks.{i}.attentions.{j}")
-                if spec.motion:
+                if spec.has_motion(f"up_blocks.{i}"):
                     add_mm(f"up_blocks.{i}.motion_modules.{j}")
             if i < nb - 1:
                 # both forms of the upsampler's conv: parity classes for an exact x2 step, the plain [Cout, 9 Cin] packing
@@ -248,15 +271,17 @@ class UNetEngine:
 
     def _pack_e4m3(self) -> Dict[str, dict]:
         """e4m3 copies (one fp32 scale per output channel, ops.pack_e4m3_weight) of the projections that read a LayerNorm
-        output: each spatial transformer's q|k|v and GEGLU, each motion module's two q|k|v and its GEGLU. The GEGLU copy is
-        quantized from the tile-interleaved pack, so its scales come in the same order."""
+        output: each spatial transformer's q|k|v and GEGLU; in every transformer block of each motion module, the q|k|v of
+        each attention block and the GEGLU. The GEGLU copy is quantized from the tile-interleaved pack, so its scales come
+        in the same order."""
         q = ops.pack_e4m3_weight
         w8: Dict[str, dict] = {}
         for p in self.xf_paths:
             w8[p] = {"qkv": q(self.w[p]["qkv"]), "geglu": q(self.w[p]["geglu"][0])}
         for p, m in self.w.items():
-            if isinstance(m, dict) and "attn" in m:
-                w8[p] = {"qkv": [q(a["qkv"]) for a in m["attn"]], "geglu": q(m["geglu"][0])}
+            if isinstance(m, dict) and "blocks" in m:
+                for k, blk in enumerate(m["blocks"]):
+                    w8[f"{p}.{k}"] = {"qkv": [q(a["qkv"]) for a in blk["attn"]], "geglu": q(blk["geglu"][0])}
         return w8
 
     def set_fp8(self, on: bool) -> None:
@@ -386,17 +411,17 @@ class UNetEngine:
     def _motion(self, p, x, b, f, hw):
         """VanillaTemporalModule (motion_module.py:77-91, 146-184, 238-261). Single GPU: f = all frames of the window.
         Frame-sharded (self.xchg, G GPUs): this GPU holds f = F / G frames; the tokens are re-sharded to pixels for the
-        transformer block (every GPU then owns all F frames of hw / G pixels, so LN + PE, q/k/v, the attention over
+        transformer blocks (every GPU then owns all F frames of hw / G pixels, so LN (+ PE), q/k/v, the attention over
         frames, out-proj and the feed-forward are all local) and back, each by one peer-memory exchange kernel."""
         m = self.w[p]
         n = b * f
         xg = self.xchg
         G = xg.G if xg is not None else 1
         F_ = f * G
-        if F_ > m["attn"][0]["pe"].shape[0]:
+        pe0 = m["blocks"][0]["attn"][0].get("pe")
+        if pe0 is not None and F_ > pe0.shape[0]:
             # the reference fails here with a shape error (motion_module.py:277-279: x + pe[:, :x.size(1)])
-            raise L.MimoError(f"{F_} frames in a window exceed temporal_position_encoding_max_len="
-                              f"{m['attn'][0]['pe'].shape[0]}")
+            raise L.MimoError(f"{F_} frames in a window exceed temporal_position_encoding_max_len={pe0.shape[0]}")
         hcur = ops.groupnorm(x, *m["gn"], n, hw, groups=self.spec.motion_groups, eps=1e-6)
         C = m["pin"][0].shape[0]
         if G == 1:
@@ -408,17 +433,20 @@ class UNetEngine:
             hw_l = hw // G
             ops.gemm(hcur, m["pin"][0], out=xg.bufs["A"].view(n * hw, C, x.dtype), bias=m["pin"][1])
             hcur = xg.pull(0, "A", torch.empty((b * F_ * hw_l, C), dtype=x.dtype, device=x.device), b, f, hw, C)
-        w8 = self.w8[p] if self.fp8 else None
-        for i, a in enumerate(m["attn"]):
-            if w8 is None:
-                nh = ops.layernorm(hcur, *a["ln"], pe=a["pe"], rows_per_frame=hw_l, frames=F_)
-                qkv = ops.gemm(nh, a["qkv"])
-            else:  # LN + PE run on this GPU's tokens after the exchange, so FP8 needs no extra communication
-                q, sc = ops.layernorm_e4m3(hcur, *a["ln"], pe=a["pe"], rows_per_frame=hw_l, frames=F_)
-                qkv = ops.gemm_e4m3(q, sc, *w8["qkv"][i], hcur.dtype)
-            att = ops.attn_temporal(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], b, F_, hw_l, self.spec.heads)
-            hcur = ops.gemm(att, a["o"][0], bias=a["o"][1], residual=hcur)
-        hcur = self._ff(hcur, m["ffn"], m["geglu"], m["ffo"], w8["geglu"] if w8 else None)
+        heads = self.spec.motion_layout.heads
+        for k, blk in enumerate(m["blocks"]):  # TemporalTransformerBlock.forward (motion_module.py:238-261)
+            w8 = self.w8[f"{p}.{k}"] if self.fp8 else None
+            for i, a in enumerate(blk["attn"]):
+                pe = a.get("pe")  # None: temporal_position_encoding off, LN alone
+                if w8 is None:
+                    nh = ops.layernorm(hcur, *a["ln"], pe=pe, rows_per_frame=hw_l, frames=F_)
+                    qkv = ops.gemm(nh, a["qkv"])
+                else:  # LN (+ PE) run on this GPU's tokens after the exchange, so FP8 needs no extra communication
+                    q, sc = ops.layernorm_e4m3(hcur, *a["ln"], pe=pe, rows_per_frame=hw_l, frames=F_)
+                    qkv = ops.gemm_e4m3(q, sc, *w8["qkv"][i], hcur.dtype)
+                att = ops.attn_temporal(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], b, F_, hw_l, heads)
+                hcur = ops.gemm(att, a["o"][0], bias=a["o"][1], residual=hcur)
+            hcur = self._ff(hcur, blk["ffn"], blk["geglu"], blk["ffo"], w8["geglu"] if w8 else None)
         if G == 1:
             return ops.gemm(hcur, m["pout"][0], bias=m["pout"][1], residual=x)
         ops.gemm(hcur, m["pout"][0], out=xg.bufs["B"].view(b * F_ * hw_l, C, x.dtype), bias=m["pout"][1])
@@ -473,7 +501,7 @@ class UNetEngine:
                 x = self._tap(f"down_blocks.{i}.resnets.{j}", self._resnet(f"down_blocks.{i}.resnets.{j}", x, None, tembs, n, h, w, rpb(h, w)), n, h, w)
                 if i < nb - 1:
                     x = self._tap(f"down_blocks.{i}.attentions.{j}", xf_fn(f"down_blocks.{i}.attentions.{j}", x, n, h * w, rpb(h, w)), n, h, w)
-                if sp.motion:
+                if sp.has_motion(f"down_blocks.{i}"):
                     x = self._tap(f"down_blocks.{i}.motion_modules.{j}", self._motion(f"down_blocks.{i}.motion_modules.{j}", x, b, f, h * w), n, h, w)
                 skips.append((x, h, w))
             if i < nb - 1:
@@ -483,7 +511,7 @@ class UNetEngine:
                 skips.append((x, h, w))
         x = self._tap("mid_block.resnets.0", self._resnet("mid_block.resnets.0", x, None, tembs, n, h, w, rpb(h, w)), n, h, w)
         x = self._tap("mid_block.attentions.0", xf_fn("mid_block.attentions.0", x, n, h * w, rpb(h, w)), n, h, w)
-        if sp.motion:
+        if sp.has_motion("mid_block"):
             x = self._tap("mid_block.motion_modules.0", self._motion("mid_block.motion_modules.0", x, b, f, h * w), n, h, w)
         x = self._tap("mid_block.resnets.1", self._resnet("mid_block.resnets.1", x, None, tembs, n, h, w, rpb(h, w)), n, h, w)
         for i in range(nb):
@@ -496,7 +524,7 @@ class UNetEngine:
                     if stop_at == pth:
                         return x, h, w
                     self._tap(pth, x, n, h, w)
-                if sp.motion:
+                if sp.has_motion(f"up_blocks.{i}"):
                     x = self._tap(f"up_blocks.{i}.motion_modules.{j}", self._motion(f"up_blocks.{i}.motion_modules.{j}", x, b, f, h * w), n, h, w)
             if i < nb - 1:
                 # the target is the skip tensor now on top of the stack (unet_3d_edit_bkfill.py:544-545)

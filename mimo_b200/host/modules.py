@@ -143,7 +143,8 @@ class _UNetBase(_EngineModel):
     _out_head = False
 
     def _init_unet(self, block_out_channels, layers_per_block, cross_attention_dim, attention_head_dim, norm_num_groups,
-                   norm_eps, in_channels, out_channels, extra: dict, motion_max_len: int = 32):
+                   norm_eps, in_channels, out_channels, extra: dict,
+                   motion_layout: schema.MotionLayout = schema.MotionLayout()):
         if isinstance(attention_head_dim, (tuple, list)):
             if len(set(attention_head_dim)) != 1:
                 raise NotImplementedError("per-level attention_head_dim is not used by the reference's SD1.5 config")
@@ -155,10 +156,11 @@ class _UNetBase(_EngineModel):
         self._spec = E.UNetSpec(block_out_channels=tuple(block_out_channels), layers_per_block=layers_per_block,
                                 heads=attention_head_dim, cross_attention_dim=cross_attention_dim,
                                 norm_num_groups=norm_num_groups, norm_eps=norm_eps, in_channels=in_channels,
-                                out_channels=out_channels, motion=self._motion, out_head=self._out_head)
+                                out_channels=out_channels, motion=self._motion, out_head=self._out_head,
+                                motion_layout=motion_layout)
         self._materialise(schema.unet_schema(block_out_channels, layers_per_block, cross_attention_dim, in_channels,
                                              out_channels, motion=self._motion, out_head=self._out_head,
-                                             motion_max_len=motion_max_len))
+                                             motion_layout=motion_layout))
         self._ref_mode: Optional[str] = None
         self._ref_cfg = False
 
@@ -228,6 +230,52 @@ class UNet2DConditionModel(_UNetBase):
         return SimpleNamespace(sample=out) if return_dict else (out,)
 
 
+# VanillaTemporalModule's defaults (motion_module.py:45-55): what an omitted motion_module_kwargs key means
+_MOTION_KW_DEFAULTS = dict(num_attention_heads=8, num_transformer_block=2,
+                           attention_block_types=("Temporal_Self", "Temporal_Self"), cross_frame_attention_mode=None,
+                           temporal_position_encoding=False, temporal_position_encoding_max_len=24,
+                           temporal_attention_dim_div=1, zero_initialize=True)
+
+
+def _motion_layout(block_out_channels, resolutions, mid_block, decoder_only, motion_module_kwargs,
+                   unsupported: list) -> schema.MotionLayout:
+    """The motion-module layout of a UNet3DConditionModel config, read as the reference reads it
+    (unet_3d_edit_bkfill.py:145-230, motion_module.py:45-144). What the engine cannot run is appended to `unsupported`."""
+    mk = dict(motion_module_kwargs or {})
+    unknown = sorted(set(mk) - set(_MOTION_KW_DEFAULTS))
+    if unknown:  # VanillaTemporalModule(**motion_module_kwargs) raises TypeError on them
+        raise TypeError(f"motion_module_kwargs: unexpected keys {unknown}")
+    mk = {**_MOTION_KW_DEFAULTS, **mk}
+    res = tuple(int(r) for r in resolutions)
+    if not set(res) <= {1, 2, 4, 8}:
+        unsupported.append(f"motion_module_resolutions={list(resolutions)} (a subset of 1, 2, 4, 8)")
+    types = list(mk["attention_block_types"])
+    if not types or any(t != "Temporal_Self" for t in types):
+        unsupported.append(f"attention_block_types={types} (one or more 'Temporal_Self'; 'Temporal_Cross' is not "
+                           "implemented)")
+    if mk["cross_frame_attention_mode"] is not None:
+        unsupported.append("cross_frame_attention_mode")
+    if mk["temporal_attention_dim_div"] != 1:
+        unsupported.append("temporal_attention_dim_div != 1")
+    blocks = int(mk["num_transformer_block"])
+    if blocks < 1:
+        unsupported.append(f"num_transformer_block={blocks} (at least 1)")
+    lay = schema.MotionLayout(resolutions=res, mid_block=bool(mid_block), decoder_only=bool(decoder_only),
+                              blocks=blocks, attn_blocks=len(types), pe=bool(mk["temporal_position_encoding"]),
+                              max_len=int(mk["temporal_position_encoding_max_len"]),
+                              heads=int(mk["num_attention_heads"]))
+    # mimo_attn_temporal runs 1 to 32 heads of at most 256 channels; a width the heads do not divide makes
+    # inner_dim != C in the reference (motion_module.py:58-61, 120-127), a different network. Head widths that are not
+    # a multiple of 8 are refused when the engine is built (UNetEngine), so that parameter containers of any width
+    # still construct, as before.
+    h = lay.heads
+    hw = lay.head_widths(block_out_channels) if h >= 1 else {}
+    if not 1 <= h <= 32 or any(d != int(d) or d > 256 for d in hw.values()):
+        unsupported.append(f"num_attention_heads={h} for motion modules of widths {sorted(hw)} (1 to 32 heads, "
+                           "dividing every width into heads of at most 256 channels)")
+    return lay
+
+
 class UNet3DConditionModel(_UNetBase):
     _motion = True
     _out_head = True
@@ -243,31 +291,28 @@ class UNet3DConditionModel(_UNetBase):
                  motion_module_decoder_only=False, motion_module_type=None, motion_module_kwargs=None,
                  unet_use_cross_frame_attention=None, unet_use_temporal_attention=None):
         super().__init__()
-        mk = dict(motion_module_kwargs or {})
-        # the engine implements the reference's shipped inference configuration (configs/inference/inference_v2.yaml)
         unsupported = []
-        if not (use_motion_module and motion_module_mid_block and not motion_module_decoder_only
-                and tuple(motion_module_resolutions) == (1, 2, 4, 8) and motion_module_type == "Vanilla"):
-            unsupported.append("motion-module placement other than inference_v2.yaml")
+        if not use_motion_module:
+            unsupported.append("use_motion_module=False (the pipeline's denoising UNet always has motion modules)")
+        if motion_module_type != "Vanilla":
+            unsupported.append(f"motion_module_type={motion_module_type!r} (only 'Vanilla')")
         if unet_use_cross_frame_attention or unet_use_temporal_attention:
             unsupported.append("unet_use_cross_frame_attention / unet_use_temporal_attention")
-        if mk.get("num_attention_heads", 8) != attention_head_dim or mk.get("num_transformer_block", 1) != 1 \
-                or list(mk.get("attention_block_types", ["Temporal_Self", "Temporal_Self"])) != ["Temporal_Self"] * 2 \
-                or not mk.get("temporal_position_encoding", True) or mk.get("temporal_attention_dim_div", 1) != 1:
-            unsupported.append("motion_module_kwargs other than inference_v2.yaml")
         if dual_cross_attention or use_linear_projection or class_embed_type or num_class_embeds or upcast_attention \
                 or resnet_time_scale_shift != "default" or center_input_sample or not flip_sin_to_cos or freq_shift:
             unsupported.append("non-SD1.5 UNet options")
+        layout = _motion_layout(block_out_channels, motion_module_resolutions, motion_module_mid_block,
+                                motion_module_decoder_only, motion_module_kwargs, unsupported)
         if unsupported:
             raise NotImplementedError("mimo_b200.UNet3DConditionModel: " + "; ".join(unsupported))
-        self._motion_max_len = mk.get("temporal_position_encoding_max_len", 32)
+        self.motion_layout = layout
         # False (the reference's default): ResnetBlock3D norm1 / norm2 and conv_norm_out are torch.nn.GroupNorm over all
         # frames of a window (resnet.py:155-163, 185-192; unet_3d_edit_bkfill.py:236-247); True: per frame
         self.use_inflated_groupnorm = bool(use_inflated_groupnorm)
         self._init_unet(block_out_channels, layers_per_block, cross_attention_dim, attention_head_dim, norm_num_groups,
                         norm_eps, 8, out_channels,  # in_channels is forced to 8 (unet_3d_edit_bkfill.py:88)
                         dict(sample_size=sample_size, use_inflated_groupnorm=self.use_inflated_groupnorm),
-                        motion_max_len=self._motion_max_len)
+                        motion_layout=layout)
         self._spec.inflated_groupnorm = self.use_inflated_groupnorm
 
     _fp8 = False

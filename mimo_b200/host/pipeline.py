@@ -15,7 +15,7 @@ sample_tensors() = _check_sampling -> CLIP -> _encode_vae -> _pose_features -> _
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Callable, Dict, List, Optional, Union
+from typing import Callable, Dict, List, Optional, Sequence, Union
 
 import numpy as np
 import PIL.Image
@@ -78,12 +78,16 @@ def _dedupe_images(images) -> "tuple[list, torch.Tensor]":
     return first, torch.tensor(inverse, dtype=torch.long)
 
 
-def shard_tokens(h: int, w: int, levels: int) -> int:
-    """Tokens per frame that every UNet level splits evenly: the gcd of h_l * w_l over the levels (engine.latent_levels).
-    A frame group of G GPUs cuts each motion module's tokens into G pixel shards, so G must divide it. For latents that
-    are multiples of 2^(levels - 1) this is the coarsest level's count; at 98 x 98 (784 x 784 pixels) it is 1."""
+def shard_tokens(h: int, w: int, levels: int, motion_levels: Optional[Sequence[int]] = None) -> int:
+    """Tokens per frame that every UNet level with a motion module splits evenly: the gcd of h_l * w_l over those levels
+    (engine.latent_levels; `motion_levels` indexes them finest first, None = every level). A frame group of G GPUs cuts
+    each motion module's tokens into G pixel shards, so G must divide it. For latents that are multiples of
+    2^(levels - 1) and modules down to the coarsest level this is that level's count; at 98 x 98 (784 x 784 pixels) it
+    is 1. Without any motion module nothing is split: 0, which every G divides."""
     import math
-    return math.gcd(*(a * b for a, b in E.latent_levels(h, w, levels)))
+    lv = E.latent_levels(h, w, levels)
+    idx = range(levels) if motion_levels is None else motion_levels
+    return math.gcd(*(lv[i][0] * lv[i][1] for i in idx))
 
 
 _POOL = None
@@ -540,8 +544,9 @@ class Pose2VideoPipeline:
             return None
         if len({len(c) for c in windows}) != 1:
             raise NotImplementedError("context windows of different lengths cannot be sharded")
+        nb = len(self.denoising_unet.config.block_out_channels)
         plan = ShardPlan.make(world, rank, do_cfg, len(windows), len(windows[0]),
-                              min_tokens=shard_tokens(h, w, len(self.denoising_unet.config.block_out_channels)))
+                              min_tokens=shard_tokens(h, w, nb, self.denoising_unet.motion_layout.levels(nb)))
         if self.force_plan is not None:
             assert self.force_plan[0] * self.force_plan[1] * self.force_plan[2] == world
             plan = ShardPlan(world, rank, *self.force_plan)

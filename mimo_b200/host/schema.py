@@ -9,7 +9,8 @@ strict=True.
 from __future__ import annotations
 
 from collections import OrderedDict
-from typing import Dict, Sequence, Tuple
+from dataclasses import dataclass
+from typing import Dict, List, Sequence, Tuple
 
 Shape = Tuple[int, ...]
 
@@ -63,24 +64,63 @@ class _S:
         self.ff(b + ".ff", c)
         self.conv(p + ".proj_out", c, c, k=1)
 
-    def motion(self, p, c, max_len):
+    def motion(self, p, c, lay: "MotionLayout"):
         t = p + ".temporal_transformer"
         self.norm(t + ".norm", c)
         self.lin(t + ".proj_in", c, c)
-        b = t + ".transformer_blocks.0"
-        for i in range(2):
-            self.attn(f"{b}.attention_blocks.{i}", c)
-            self.d[f"{b}.attention_blocks.{i}.pos_encoder.pe"] = (1, max_len, c)
-            self.norm(f"{b}.norms.{i}", c)
-        self.ff(b + ".ff", c)
-        self.norm(b + ".ff_norm", c)
+        for k in range(lay.blocks):
+            b = f"{t}.transformer_blocks.{k}"
+            for i in range(lay.attn_blocks):
+                self.attn(f"{b}.attention_blocks.{i}", c)
+                if lay.pe:
+                    self.d[f"{b}.attention_blocks.{i}.pos_encoder.pe"] = (1, lay.max_len, c)
+                self.norm(f"{b}.norms.{i}", c)
+            self.ff(b + ".ff", c)
+            self.norm(b + ".ff_norm", c)
         self.lin(t + ".proj_out", c, c)
+
+
+@dataclass(frozen=True)
+class MotionLayout:
+    """Where the denoising UNet3D has a VanillaTemporalModule and what each one holds (unet_3d_edit_bkfill.py:145-230,
+    motion_module.py:45-55, 98-144, 212-236). The defaults are configs/inference/inference_v2.yaml's."""
+    resolutions: Tuple[int, ...] = (1, 2, 4, 8)  # motion_module_resolutions
+    mid_block: bool = True                        # motion_module_mid_block
+    decoder_only: bool = False                    # motion_module_decoder_only
+    blocks: int = 1                               # num_transformer_block
+    attn_blocks: int = 2                          # len(attention_block_types), all "Temporal_Self"
+    pe: bool = True                               # temporal_position_encoding
+    max_len: int = 32                             # temporal_position_encoding_max_len
+    heads: int = 8                                # num_attention_heads
+
+    def placed(self, path: str, levels: int) -> bool:
+        """Whether the block at `path` ("down_blocks.i", "mid_block" or "up_blocks.i") has motion modules. Down level i
+        is resolution 2^i, up level i is 2^(3 - i) whatever the number of levels, as the reference computes them
+        (unet_3d_edit_bkfill.py:124, 188)."""
+        if path == "mid_block":
+            return self.mid_block
+        kind, i = path.split(".")
+        if kind == "down_blocks":
+            return not self.decoder_only and 2 ** int(i) in self.resolutions
+        return 2 ** (3 - int(i)) in self.resolutions
+
+    def levels(self, levels: int) -> List[int]:
+        """The UNet levels (0 = finest) at which some block has motion modules."""
+        return [lv for lv in range(levels) if self.placed(f"down_blocks.{lv}", levels)
+                or self.placed(f"up_blocks.{levels - 1 - lv}", levels) or (lv == levels - 1 and self.mid_block)]
+
+    def head_widths(self, block_out_channels: Sequence[int]) -> Dict[int, float]:
+        """{module width: channels per temporal-attention head} over the levels that have motion modules"""
+        ch = list(block_out_channels)
+        return {ch[lv]: ch[lv] / self.heads for lv in self.levels(len(ch))}
 
 
 def unet_schema(block_out_channels: Sequence[int] = (320, 640, 1280, 1280), layers_per_block: int = 2,
                 cross_attention_dim: int = 768, in_channels: int = 8, out_channels: int = 4, motion: bool = True,
-                out_head: bool = True, motion_max_len: int = 32) -> Dict[str, Shape]:
+                out_head: bool = True, motion_layout: MotionLayout = MotionLayout()) -> Dict[str, Shape]:
+    """motion: the denoising UNet3D, with motion modules where `motion_layout` places them; False: the UNet2D."""
     s = _S()
+    lay = motion_layout
     ch = list(block_out_channels)
     nb = len(ch)
     temb = ch[0] * 4
@@ -94,14 +134,14 @@ def unet_schema(block_out_channels: Sequence[int] = (320, 640, 1280, 1280), laye
             s.resnet(f"down_blocks.{i}.resnets.{j}", in_c if j == 0 else out_c, out_c, temb)
             if i < nb - 1:
                 s.xf(f"down_blocks.{i}.attentions.{j}", out_c, cross_attention_dim)
-            if motion:
-                s.motion(f"down_blocks.{i}.motion_modules.{j}", out_c, motion_max_len)
+            if motion and lay.placed(f"down_blocks.{i}", nb):
+                s.motion(f"down_blocks.{i}.motion_modules.{j}", out_c, lay)
         if i < nb - 1:
             s.conv(f"down_blocks.{i}.downsamplers.0.conv", out_c, out_c)
     s.resnet("mid_block.resnets.0", ch[-1], ch[-1], temb)
     s.xf("mid_block.attentions.0", ch[-1], cross_attention_dim)
-    if motion:
-        s.motion("mid_block.motion_modules.0", ch[-1], motion_max_len)
+    if motion and lay.placed("mid_block", nb):
+        s.motion("mid_block.motion_modules.0", ch[-1], lay)
     s.resnet("mid_block.resnets.1", ch[-1], ch[-1], temb)
     rev = ch[::-1]
     out_c = rev[0]
@@ -114,8 +154,8 @@ def unet_schema(block_out_channels: Sequence[int] = (320, 640, 1280, 1280), laye
             s.resnet(f"up_blocks.{i}.resnets.{j}", res_in + skip_c, out_c, temb)
             if i > 0:
                 s.xf(f"up_blocks.{i}.attentions.{j}", out_c, cross_attention_dim)
-            if motion:
-                s.motion(f"up_blocks.{i}.motion_modules.{j}", out_c, motion_max_len)
+            if motion and lay.placed(f"up_blocks.{i}", nb):
+                s.motion(f"up_blocks.{i}.motion_modules.{j}", out_c, lay)
         if i < nb - 1:
             s.conv(f"up_blocks.{i}.upsamplers.0.conv", out_c, out_c)
     if out_head:

@@ -27,6 +27,9 @@ def main():
     ap.add_argument("--frames", type=int, nargs="*", default=None, help="only the cases with these frame counts")
     ap.add_argument("--window-groupnorm", action="store_true",
                     help="denoising UNet built with use_inflated_groupnorm=False (ResBlock GroupNorms over the window)")
+    ap.add_argument("--motion-layout", default=None, choices=["v1", "v3", "stress", "omitted"],
+                    help="denoising UNet with this motion-module layout of oracle/gen_motion_layout_golden.py (its own "
+                         "use_inflated_groupnorm) instead of inference_v2.yaml's")
     args = ap.parse_args()
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     torch.cuda.set_device(local)
@@ -57,14 +60,23 @@ def main():
     seed = 700
     mk = dict(num_attention_heads=8, num_transformer_block=1, attention_block_types=["Temporal_Self", "Temporal_Self"],
               temporal_position_encoding=True, temporal_position_encoding_max_len=32, temporal_attention_dim_div=1)
-    den = M.UNet3DConditionModel(block_out_channels=widths, cross_attention_dim=768,
-                                 use_inflated_groupnorm=not args.window_groupnorm,
-                                 use_motion_module=True, motion_module_mid_block=True, motion_module_type="Vanilla",
-                                 motion_module_kwargs=mk)
+    if args.motion_layout is None:
+        den = M.UNet3DConditionModel(block_out_channels=widths, cross_attention_dim=768,
+                                     use_inflated_groupnorm=not args.window_groupnorm,
+                                     use_motion_module=True, motion_module_mid_block=True, motion_module_type="Vanilla",
+                                     motion_module_kwargs=mk)
+        sd_den = O.make_denoising_unet_sd(cfg, seed)
+    else:
+        from oracle import gen_motion_layout_golden as GL
+        from oracle import motion_layout_oracle as ML
+        lay = next(c for c in GL.LAYOUTS if c["name"] == args.motion_layout)
+        den = M.UNet3DConditionModel(block_out_channels=widths, cross_attention_dim=768, use_motion_module=True,
+                                     motion_module_type="Vanilla", **lay["kwargs"])
+        sd_den = ML.make_denoising_unet_sd(cfg, lay["layout"], seed)
     ref = M.UNet2DConditionModel(block_out_channels=widths, cross_attention_dim=768)
     pg = M.PoseGuider(widths[0], 3, (16, 32, 96, 256))
     vae = M.AutoencoderKL()
-    den.load_state_dict(O.make_denoising_unet_sd(cfg, seed))
+    den.load_state_dict(sd_den)
     ref.load_state_dict(O.make_reference_unet_sd(cfg, seed + 1))
     pg.load_state_dict(O.make_pose_guider_sd(seed + 2, widths[0]))
     vae.load_state_dict(O.make_vae_sd(vcfg, seed + 3))
@@ -102,10 +114,11 @@ def main():
         b2 = run()
         b3 = run()  # eager, capture, replay
         same_sh = bool(torch.equal(lat_b, pipe.last_latents) and torch.equal(b1, b3) and torch.equal(b1, b2))
-        from mimo_b200.host.shard import ShardPlan
         from mimo_b200.host.context import uniform
+        from mimo_b200.host.pipeline import shard_tokens
+        from mimo_b200.host.shard import ShardPlan
         plan = ShardPlan.make(world, rank, guidance > 1.0, len(list(uniform(0, 2, F_, 24, 1, 4))), 24,
-                              min_tokens=(size // 64) ** 2)
+                              min_tokens=shard_tokens(size // 8, size // 8, 4, den.motion_layout.levels(4)))
         if forced is not None:
             plan = ShardPlan(world, rank, *forced)
         row = {"F": F_, "cfg": guidance > 1.0, "plan": [plan.cfg_ways, plan.win_ways, plan.frame_ways],
