@@ -41,9 +41,8 @@ const char* mimo_last_error(void);
 /* 0 if device `dev` is sm_90; MIMO_ERR_DEVICE otherwise (also when there is no CUDA device at all). */
 int mimo_device_check(int dev);
 /* sizeof() of the parameter structs as compiled into the library (0 epilogue, 1 gemm, 2 conv3x3, 3 groupnorm,
- * 4 attn, 5 attn_temporal, 6 exchange, 7 cfg_multistep, 8 groupnorm_window, 9 gemm_e4m3): lets a binding verify its
- * struct mirrors
- * before the first call. */
+ * 4 attn, 5 attn_temporal, 6 exchange, 7 cfg_multistep, 8 groupnorm_window, 9 gemm_e4m3, 10 groupnorm_e4m3,
+ * 11 conv3x3_e4m3): lets a binding verify its struct mirrors before the first call. */
 int mimo_abi_sizeof(int which);
 
 /* Fused epilogue shared by GEMM and conv:  out = act((acc + bias[c] + rowvec[row / rows_per_group][c]
@@ -146,6 +145,32 @@ int mimo_conv3x3(const mimo_conv3x3_params* p, void* stream);
  * (mimo_b200.ops.pack_conv_up2x_weight). Epilogue: bias / scale / SiLU only. */
 int mimo_conv_up2x(const mimo_conv3x3_params* p, void* stream);
 
+/* FP8 form of mimo_conv3x3 for convolutions fed by mimo_groupnorm_e4m3:
+ *   out[n, y, x, o] = epilogue((sum_{tap, c} X[n, y + dy, x + dx, c] * W[o, tap * c_in + c]) * x_scale[n] * w_scale[o])
+ * X and W are e4m3 (OCP E4M3FN), x_scale one fp32 scale per image (a tap never leaves its image, and padding is zero, so
+ * the scale factors out of every output pixel's sum), w_scale one per output channel; accumulation in fp32. The product
+ * with the two scales is taken in fp32 in that order, then the mimo_epilogue chain runs as in mimo_conv3x3 (bias, rowvec,
+ * residual, act NONE or SILU, scale); out, bias, rowvec and residual are `dtype` (fp16 / bf16).
+ * Replaces, when the caller opts into FP8 convolutions, ResnetBlock3D's conv1 and conv2 (InflatedConv3d,
+ * src/models/resnet.py:9-17, called at resnet.py:222 and :239). Single source (mimo_groupnorm_e4m3 writes the up blocks'
+ * channel concat). Requirements: c_in % 16 == 0, cout % 8 == 0, ldo % 8 == 0, 16-byte aligned x / w / out / residual,
+ * non-NULL scales, no GEGLU, no split-K (workspace must be NULL). */
+typedef struct {
+  const void* x;        /* [n, h, w_, c_in] e4m3 */
+  const float* x_scale; /* [n] */
+  int32_t c_in;
+  const void* w;        /* [cout, 9 * c_in] e4m3, K index = tap * c_in + channel as in mimo_conv3x3 */
+  const float* w_scale; /* [cout] */
+  void* out;
+  int64_t ldo;
+  int32_t n, h, w_, cout;
+  int32_t dtype; /* of out / bias / rowvec / residual */
+  mimo_epilogue ep;
+  void* workspace; /* must be NULL */
+  int64_t workspace_bytes;
+} mimo_conv3x3_e4m3_params;
+int mimo_conv3x3_e4m3(const mimo_conv3x3_e4m3_params* p, void* stream);
+
 /* im2col gather for the convolutions the TMA path does not cover (stride 2, nearest-x2 upsampled input):
  * col[(n,oy,ox), tap*c + ch] = x[n, (oy*stride-1+ky) >> up, (ox*stride-1+kx) >> up, ch], zero outside.
  * Replaces: Downsample3D (src/models/resnet.py:112-120), F.interpolate in Upsample3D (resnet.py:70-73),
@@ -209,6 +234,53 @@ int mimo_groupnorm_window_apply(const mimo_groupnorm_window_params* p, void* str
 /* bytes of the partial table of x's `frames` frames (pointers and table_frames ignored); < 0 on bad sizes. The table of
  * a window sharded into G equal frame slices is G times the slice's. */
 int64_t mimo_groupnorm_window_table_bytes(const mimo_groupnorm_window_params* p);
+
+/* GroupNorm + SiLU with an e4m3 output and one fp32 scale per image: the A operand of mimo_conv3x3_e4m3.
+ * Replaces, when the caller opts into FP8 convolutions, ResnetBlock3D's norm1 / norm2 + SiLU ahead of conv1 / conv2
+ * (src/models/resnet.py:217-240; InflatedGroupNorm resnet.py:20-28, or nn.GroupNorm over the window, resnet.py:155-163).
+ * The scale is an upper bound on the image's amax, built before any output is written. For image i and group g, with
+ * lo_g / hi_g the min / max of x over the image's elements of the group, mean_g / rstd_g the normaliser's statistics
+ * (the image's own, or the sample's window statistics), and for each channel c of g
+ *   z_lo = (lo_g - mean_g) * (rstd_g * gamma_c) + beta_c,  z_hi likewise with hi_g  (one fma each, as the normaliser)
+ *   B_c = max(|silu(z_lo)|, |silu(z_hi)|, and 0.27846454 when [min(z_lo, z_hi), max(z_lo, z_hi)] holds -1.2784645)
+ *   amax_i = max_c B_c;  scale[i] = amax_i / 448,  out = cvt.rn.satfinite.e4m3(silu(y) * (448 / amax_i))  (IEEE divisions)
+ * and scale[i] = 1, multiplier 1 when amax_i == 0. SiLU's only turning point is its minimum at -1.2784645, so B_c bounds
+ * |silu| over [z_lo, z_hi]: nothing saturates except by rounding. mimo_b200.ops.e4m3_image_scales states the rule on the
+ * host. x, gamma, beta are `dtype`; out is [samples * frames, hw, c0 + c1] bytes (image = sample * frames + frame).
+ * Modes (the window modes keep mimo_groupnorm_window's partial table and its format; min / max never enter the table, so
+ * a frame-sharded window exchanges exactly what the 16-bit GroupNorm exchanges):
+ *   MIMO_GN_E4M3_FRAME          statistics per image (`table` unused)
+ *   MIMO_GN_E4M3_WINDOW         statistics per sample over its `frames` frames, both passes (table of `frames` records)
+ *   MIMO_GN_E4M3_WINDOW_PARTIALS the `frames` records of x's frames into `table`, the min / max into `work`
+ *   MIMO_GN_E4M3_WINDOW_APPLY   normalise x's frames from a table of table_frames >= frames records, with the min / max
+ *                               the partials call left in `work`
+ * work: scratch of mimo_groupnorm_e4m3_workspace_bytes(p) bytes, 16-byte aligned (kept between PARTIALS and APPLY).
+ * Requirements: as mimo_groupnorm_window; silu is implied. All modes are graph-capturable. */
+#define MIMO_GN_E4M3_FRAME 0
+#define MIMO_GN_E4M3_WINDOW 1
+#define MIMO_GN_E4M3_WINDOW_PARTIALS 2
+#define MIMO_GN_E4M3_WINDOW_APPLY 3
+typedef struct {
+  const void* x0;
+  int32_t c0;
+  const void* x1; /* NULL if single source */
+  int32_t c1;
+  const void* gamma;
+  const void* beta;    /* [c0 + c1] */
+  void* out;           /* [samples * frames, hw, c0 + c1] e4m3 */
+  float* scale;        /* [samples * frames] */
+  float* work;
+  int64_t work_bytes;
+  float* table;        /* window modes: partial table as in mimo_groupnorm_window */
+  int64_t table_bytes;
+  int32_t mode;
+  int32_t samples, frames, table_frames, hw, groups;
+  float eps;
+  int32_t dtype;
+} mimo_groupnorm_e4m3_params;
+int mimo_groupnorm_e4m3(const mimo_groupnorm_e4m3_params* p, void* stream);
+/* bytes of `work` for these sizes and mode (pointers ignored); < 0 on bad sizes */
+int64_t mimo_groupnorm_e4m3_workspace_bytes(const mimo_groupnorm_e4m3_params* p);
 
 /* LayerNorm over the last dim; optional additive per-frame vector AFTER the affine (the motion module's
  * sinusoidal positional encoding): out[r] = LN(x[r]) * gamma + beta + pe[pe_frame_offset + (r / rows_per_frame) % frames]

@@ -109,6 +109,8 @@ extern "C" int mimo_abi_sizeof(int which) {
     case 7: return static_cast<int>(sizeof(mimo_cfg_multistep_params));
     case 8: return static_cast<int>(sizeof(mimo_groupnorm_window_params));
     case 9: return static_cast<int>(sizeof(mimo_gemm_e4m3_params));
+    case 10: return static_cast<int>(sizeof(mimo_groupnorm_e4m3_params));
+    case 11: return static_cast<int>(sizeof(mimo_conv3x3_e4m3_params));
   }
   return -1;
 }

@@ -18,9 +18,10 @@
 // (tap, 64-channel block, source tensor); TMA's out-of-bounds zero fill is the conv's zero padding and also
 // the K tail, and the output / residual boxes use the same {TW, TH, TN} footprint (stores are clipped at image
 // borders). Two source tensors give the up-blocks' channel concat without materialising it.
-// E4M3 mode (mimo_gemm_e4m3, GEMM rows only) runs the same roles on fp8 A and W: a K block is 128 one-byte elements, the
+// E4M3 mode (mimo_gemm_e4m3, GEMM rows) runs the same roles on fp8 A and W: a K block is 128 one-byte elements, the
 // same 128-byte swizzle row and stage bytes, four wgmma.m64nBNk32.e4m3 per block; the epilogue first takes
-// acc * a_scale[row] * w_scale[col] in fp32 and then runs the chain above unchanged.
+// acc * a_scale[row] * w_scale[col] in fp32 and then runs the chain above unchanged. mimo_conv3x3_e4m3 is conv mode in
+// e4m3 (conv_e4m3_kernel): 128-channel boxes, single source, and a_scale per image of the output pixel.
 #include <cuda_runtime.h>
 
 #include <cudaTypedefs.h>
@@ -88,7 +89,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
                   const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOut,
                   const __grid_constant__ CUtensorMap tmRes, int M, int N, int num_m_tiles, int num_n_tiles,
                   int num_k_blocks, ConvGeom g, EpiArgs ep) {
-  constexpr bool kE4m3 = false;
+  constexpr bool kE4m3 = false, kImgScale = false;
   constexpr const float* a_scale = nullptr;
   constexpr const float* w_scale = nullptr;
 #include "gemm_wgmma_body.cuh"
@@ -103,7 +104,20 @@ gemm_e4m3_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
                  const __grid_constant__ CUtensorMap tmRes, int M, int N, int num_m_tiles, int num_n_tiles,
                  int num_k_blocks, ConvGeom g, EpiArgs ep, const float* __restrict__ a_scale,
                  const float* __restrict__ w_scale) {
-  constexpr bool kE4m3 = true;
+  constexpr bool kE4m3 = true, kImgScale = false;
+#include "gemm_wgmma_body.cuh"
+}
+
+// e4m3 3x3 convolution (g.conv == 1, single source: tmA1 == tmA0 and kb1 == 0, no split-K): as gemm_e4m3_kernel, with
+// a_scale one fp32 scale per IMAGE, read for each tile row from the image its output pixel lies in
+template <int BN, bool kBf16, bool kRes>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+conv_e4m3_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
+                 const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOut,
+                 const __grid_constant__ CUtensorMap tmRes, int M, int N, int num_m_tiles, int num_n_tiles,
+                 int num_k_blocks, ConvGeom g, EpiArgs ep, const float* __restrict__ a_scale,
+                 const float* __restrict__ w_scale) {
+  constexpr bool kE4m3 = true, kImgScale = true;
 #include "gemm_wgmma_body.cuh"
 }
 
@@ -238,6 +252,8 @@ int pick_bn(int N, bool geglu, long long m_tiles);
 //   gemm_e4m3_kernel<192, *, *>: 144-155 registers, no spills
 //   gemm_e4m3_kernel<256, f16 / bf16, no residual>: 168 registers, 32 / 16 B spill stores, 36 / 20 B spill loads
 //   gemm_e4m3_kernel<256, *, residual>: 168 registers, 32 B spill stores, 48 B spill loads
+//   conv_e4m3_kernel<160, *, no residual / residual>: 128 / 144-148 registers, no spills
+//   conv_e4m3_kernel<256, *, *>: as gemm_e4m3_kernel<256, *, *> (the engine uses it for 1280 channels at 8 x 8)
 //   (gemm_wgmma_kernel<256, *, *>, for comparison: 168 registers, 8 B spill stores, 8-16 B spill loads)
 // e4m3 tile widths (gemm_e4m3_kernel instantiations): 192 and 256 are the widths pick_bn gives the LN-fed GEMMs of the
 // UNet (q|k|v N = 3 C: 960 / 1920 -> 192, 3840 -> 256; GEGLU N = 8 C -> 256).
@@ -486,6 +502,25 @@ extern "C" int mimo_gemm_e4m3(const mimo_gemm_e4m3_params* p, void* stream) {
                                : launch_e4m3<false>(bn, res, m, p->M, p->N, mt, nt, nkb, g, ep, p->a_scale, p->w_scale, st);
 }
 
+// conv mode and the {TW, TH, TN} output footprint of a 128-row tile over [n, h, w] images; returns the tiles along n
+static int conv_tiles(ConvGeom& g, int n, int h, int w) {
+  g.conv = 1;
+  g.H = h;
+  g.W = w;
+  g.NI = n;
+  g.TW = w < BM ? w : BM;
+  g.TH = BM / g.TW;
+  if (g.TH > h) g.TH = h;
+  if (g.TH < 1) g.TH = 1;
+  g.TN = BM / (g.TW * g.TH);
+  if (g.TN > n) g.TN = n;
+  if (g.TN < 1) g.TN = 1;
+  if (g.TN > 1 && g.TH != h) g.TN = 1;  // several images per tile only when a tile spans whole images
+  g.tiles_w = (w + g.TW - 1) / g.TW;
+  g.tiles_h = (h + g.TH - 1) / g.TH;
+  return (n + g.TN - 1) / g.TN;
+}
+
 // One implicit-GEMM convolution launch: `ntaps` taps at offsets (tdx, tdy) over the [n, h, w, c] input(s); the output
 // (and residual) pixel (n, y, x) lives at out + ((n * oh + y * sy) * ow + x * sx) * ldo elements, i.e. a strided view of a
 // larger image when (sx, sy) != (1, 1).
@@ -493,21 +528,7 @@ static int conv_launch(const mimo_conv3x3_params* p, const void* w, int ntaps, c
                        const signed char* tdy, void* out, int sx, int sy, int ow, int oh, void* stream) {
   const int c1 = p->x1 ? p->c1 : 0;
   ConvGeom g = {};
-  g.conv = 1;
-  g.H = p->h;
-  g.W = p->w_;
-  g.NI = p->n;
-  g.TW = p->w_ < BM ? p->w_ : BM;
-  g.TH = BM / g.TW;
-  if (g.TH > p->h) g.TH = p->h;
-  if (g.TH < 1) g.TH = 1;
-  g.TN = BM / (g.TW * g.TH);
-  if (g.TN > p->n) g.TN = p->n;
-  if (g.TN < 1) g.TN = 1;
-  if (g.TN > 1 && g.TH != p->h) g.TN = 1;  // several images per tile only when a tile spans whole images
-  g.tiles_w = (p->w_ + g.TW - 1) / g.TW;
-  g.tiles_h = (p->h + g.TH - 1) / g.TH;
-  const int tiles_n = (p->n + g.TN - 1) / g.TN;
+  const int tiles_n = conv_tiles(g, p->n, p->h, p->w_);
   g.ctot = p->c0 + c1;
   g.c0 = p->c0;
   g.kb0 = (p->c0 + BK - 1) / BK;
@@ -619,4 +640,122 @@ extern "C" int mimo_conv_up2x(const mimo_conv3x3_params* p, void* stream) {
       if (int rc = conv_launch(p, w, 4, dx, dy, out, 2, 2, 2 * p->w_, 2 * p->h, stream)) return rc;
     }
   return MIMO_OK;
+}
+
+// e4m3 conv tile widths (conv_e4m3_kernel instantiations): 160 divides every ResBlock width (320, 640, 1280), 256 divides
+// 1280. At 1280 BN 256 spills (ptxas report above) and 160 does not; measured on an H100 SXM (700 W) at the 48 images of
+// the 512 x 512 CFG window, 256 was faster where its tiles fit one wave and 160's did not (8 x 8: 66 / 68 / 123 us
+// against 83 / 85 / 152 us), and at 16 x 16 the two were within 8 % either way (scripts/fp8_conv_bench.py). So: 256 when
+// that saves a wave, else the least padded width, 160 on a tie.
+static int pick_bn_conv_e4m3(int N, long long m_tiles) {
+  if (g_force_bn) return g_force_bn;
+  const long long t256 = m_tiles * ((N + 255) / 256), t160 = m_tiles * ((N + 159) / 160);
+  if (N % 256 == 0 && t256 <= num_sms() && t160 > num_sms()) return 256;
+  const int pad256 = (N + 255) / 256 * 256 - N, pad160 = (N + 159) / 160 * 160 - N;
+  return pad256 < pad160 ? 256 : 160;
+}
+
+template <int BN, bool kBf16, bool kRes>
+static int launch_conv_e4m3_cfg(const Maps& m, int M, int N, int mt, int nt, int nkb, const ConvGeom& g,
+                                const EpiArgs& ep, const float* a_scale, const float* w_scale, cudaStream_t st) {
+  constexpr int kSmem = GemmCfg<BN, kRes, true>::kSmemBytes;
+  auto kern = conv_e4m3_kernel<BN, kBf16, kRes>;
+  static bool attr_done = false;  // per instantiation
+  if (!attr_done) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
+    if (e != cudaSuccess) return set_cuda_error("cudaFuncSetAttribute(conv_e4m3)", e);
+    attr_done = true;
+  }
+  const int tiles = mt * nt;
+  const int grid = tiles < num_sms() ? tiles : num_sms();
+  cudaError_t e = launch_k(kern, dim3(grid), dim3(kGemmThreads), kSmem, st, m.a0, m.a1, m.b, m.out, m.res, M, N, mt, nt,
+                           nkb, g, ep, a_scale, w_scale);
+  if (e == cudaSuccess) e = cudaGetLastError();
+  if (e != cudaSuccess) return set_cuda_error("conv_e4m3 launch", e);
+  return MIMO_OK;
+}
+
+template <bool kBf16>
+static int launch_conv_e4m3(int bn, bool res, const Maps& m, int M, int N, int mt, int nt, int nkb, const ConvGeom& g,
+                            const EpiArgs& ep, const float* a_scale, const float* w_scale, cudaStream_t st) {
+  if (bn == 160)
+    return res ? launch_conv_e4m3_cfg<160, kBf16, true>(m, M, N, mt, nt, nkb, g, ep, a_scale, w_scale, st)
+               : launch_conv_e4m3_cfg<160, kBf16, false>(m, M, N, mt, nt, nkb, g, ep, a_scale, w_scale, st);
+  return res ? launch_conv_e4m3_cfg<256, kBf16, true>(m, M, N, mt, nt, nkb, g, ep, a_scale, w_scale, st)
+             : launch_conv_e4m3_cfg<256, kBf16, false>(m, M, N, mt, nt, nkb, g, ep, a_scale, w_scale, st);
+}
+
+extern "C" int mimo_conv3x3_e4m3(const mimo_conv3x3_e4m3_params* p, void* stream) {
+  if (!p || !p->x || !p->w || !p->out || !p->x_scale || !p->w_scale)
+    return set_error(MIMO_ERR_ARG, "mimo_conv3x3_e4m3: null pointer");
+  if (p->n <= 0 || p->h <= 0 || p->w_ <= 0 || p->cout <= 0 || p->c_in <= 0)
+    return set_error(MIMO_ERR_ARG, "mimo_conv3x3_e4m3: empty problem");
+  if (p->c_in % 16) return set_error(MIMO_ERR_ARG, "mimo_conv3x3_e4m3: c_in must be a multiple of 16");
+  if ((p->cout % 8) || (p->ldo % 8)) return set_error(MIMO_ERR_ARG, "mimo_conv3x3_e4m3: cout, ldo must be multiples of 8");
+  if ((reinterpret_cast<uintptr_t>(p->x) | reinterpret_cast<uintptr_t>(p->w) | reinterpret_cast<uintptr_t>(p->out) |
+       reinterpret_cast<uintptr_t>(p->ep.residual)) % 16)
+    return set_error(MIMO_ERR_ARG, "mimo_conv3x3_e4m3: x, w, out, residual must be 16-byte aligned");
+  if (p->ep.residual && (p->ep.ld_res % 8)) return set_error(MIMO_ERR_ARG, "mimo_conv3x3_e4m3: ld_res % 8 != 0");
+  if (p->ep.act == MIMO_ACT_GEGLU) return set_error(MIMO_ERR_ARG, "mimo_conv3x3_e4m3: GEGLU not supported");
+  if (p->workspace || p->workspace_bytes) return set_error(MIMO_ERR_ARG, "mimo_conv3x3_e4m3: split-K is not supported");
+  const long long Mrows = static_cast<long long>(p->n) * p->h * p->w_;
+  if (Mrows > 0x7fffffffLL) return set_error(MIMO_ERR_ARG, "mimo_conv3x3_e4m3: too many pixels");
+  if (g_force_bn && g_force_bn != 160 && g_force_bn != 256)
+    return set_error(MIMO_ERR_ARG, "mimo_conv3x3_e4m3: unsupported BN (160 or 256)");
+  if (int rc = ensure_device()) return rc;
+
+  ConvGeom g = {};
+  const int tiles_n = conv_tiles(g, p->n, p->h, p->w_);
+  const int bn = pick_bn_conv_e4m3(p->cout, static_cast<long long>(g.tiles_w) * g.tiles_h * tiles_n);
+  g.ctot = g.c0 = p->c_in;
+  g.kb0 = (p->c_in + 2 * BK - 1) / (2 * BK);  // 128-channel blocks per tap
+  g.a_bytes = g.TW * g.TH * g.TN * 2 * BK;
+  g.chunk_bytes = g.TW * g.TH * g.TN * 64;
+  g.ntaps = 9;
+  for (int t = 0; t < 9; ++t) {
+    g.tdx[t] = static_cast<signed char>(t % 3 - 1);
+    g.tdy[t] = static_cast<signed char>(t / 3 - 1);
+  }
+  const int mt = g.tiles_w * g.tiles_h * tiles_n;
+  const int nkb = 9 * g.kb0;
+  g.splits = 1;
+  g.kb_split = nkb;
+  const int nt = (p->cout + bn - 1) / bn;
+  const bool res = p->ep.residual != nullptr;
+
+  Maps m;
+  const uint32_t tile[3] = {static_cast<uint32_t>(g.TW), static_cast<uint32_t>(g.TH), static_cast<uint32_t>(g.TN)};
+  {
+    const uint64_t dim[4] = {static_cast<uint64_t>(p->c_in), static_cast<uint64_t>(p->w_), static_cast<uint64_t>(p->h),
+                             static_cast<uint64_t>(p->n)};
+    const uint64_t str[3] = {static_cast<uint64_t>(p->c_in), static_cast<uint64_t>(p->w_) * p->c_in,
+                             static_cast<uint64_t>(p->h) * p->w_ * p->c_in};
+    const uint32_t box[4] = {2 * BK, tile[0], tile[1], tile[2]};
+    if (int rc = encode_tmap(&m.a0, kTmapU8, 4, p->x, dim, str, box)) return rc;
+    m.a1 = m.a0;
+  }
+  {
+    const uint64_t dim[2] = {9ull * p->c_in, static_cast<uint64_t>(p->cout)};
+    const uint64_t str[1] = {9ull * p->c_in};
+    const uint32_t box[2] = {2 * BK, static_cast<uint32_t>(bn)};
+    if (int rc = encode_tmap(&m.b, kTmapU8, 2, p->w, dim, str, box)) return rc;
+  }
+  auto out_map = [&](CUtensorMap* tm, const void* base, long long pitch) {
+    const uint64_t dim[4] = {static_cast<uint64_t>(p->cout), static_cast<uint64_t>(p->w_), static_cast<uint64_t>(p->h),
+                             static_cast<uint64_t>(p->n)};
+    const uint64_t str[3] = {static_cast<uint64_t>(pitch) * 2, static_cast<uint64_t>(p->w_) * pitch * 2,
+                             static_cast<uint64_t>(p->h) * p->w_ * pitch * 2};
+    const uint32_t box[4] = {32, tile[0], tile[1], tile[2]};
+    return encode_tmap(tm, p->dtype, 4, base, dim, str, box, 64);
+  };
+  if (int rc = out_map(&m.out, p->out, p->ldo)) return rc;
+  m.res = m.out;
+  if (res)
+    if (int rc = out_map(&m.res, p->ep.residual, p->ep.ld_res)) return rc;
+  const EpiArgs ep = make_epi(p->ep, p->cout);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int M = static_cast<int>(Mrows);
+  return p->dtype == MIMO_BF16
+             ? launch_conv_e4m3<true>(bn, res, m, M, p->cout, mt, nt, nkb, g, ep, p->x_scale, p->w_scale, st)
+             : launch_conv_e4m3<false>(bn, res, m, M, p->cout, mt, nt, nkb, g, ep, p->x_scale, p->w_scale, st);
 }

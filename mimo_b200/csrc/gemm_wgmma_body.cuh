@@ -1,10 +1,12 @@
 // Body of the GEMM / conv kernels of gemm_wgmma.cu (see the description at the top of that file). Not a header: the
 // kernels there include it as their whole body, so the 16-bit kernel is compiled from the same statements with the e4m3
 // steps removed by `if constexpr (kE4m3)`, and keeps its parameter list and generated code. In scope at the include:
-// the template parameters BN, kBf16, kRes, the constant kE4m3, the kernel parameters tmA0, tmA1, tmB, tmOut, tmRes, M, N,
-// num_m_tiles, num_n_tiles, num_k_blocks, g, ep, and a_scale, w_scale (fp32 row scales of A and W, used when kE4m3).
+// the template parameters BN, kBf16, kRes, the constants kE4m3 and kImgScale, the kernel parameters tmA0, tmA1, tmB, tmOut,
+// tmRes, M, N, num_m_tiles, num_n_tiles, num_k_blocks, g, ep, and a_scale, w_scale (fp32 scales of A and W, used when
+// kE4m3: a_scale per A row, or with kImgScale per image of a convolution).
   using Cfg = GemmCfg<BN, kRes, kE4m3>;
   constexpr int kBKel = kE4m3 ? 2 * BK : BK;  // elements per K block (one 128-byte swizzle row either way)
+  constexpr int kConvKel = kImgScale ? kBKel : BK;  // channels per conv K block (gemm_e4m3_kernel runs GEMM rows only)
   using C = Cvt<kBf16>;
   using T = typename C::T;
   constexpr int NCHUNK = Cfg::kNChunk;
@@ -98,12 +100,15 @@
           } else {
             mbar_expect_tx(&full_bar[stage], g.a_bytes + BN * BK * 2);
             int kcoord;
+            // e4m3: a channel count of 64 mod 128 (320, 960) leaves half a block in each tap; TMA zero-fills the A box
+            // past the channels, while the W box reads on into the next tap's weights (finite e4m3 bytes): they meet
+            // zeros only, so the sum is exact, at 384 / 320 of the MMA work for 320 channels
             if (rem < g.kb0) {
-              tma_load_4d(sa, &tmA0, &full_bar[stage], rem * BK, x0 + dx, y0 + dy, n0);
-              kcoord = tap_k + rem * BK;
+              tma_load_4d(sa, &tmA0, &full_bar[stage], rem * kConvKel, x0 + dx, y0 + dy, n0);
+              kcoord = tap_k + rem * kConvKel;
             } else {
-              tma_load_4d(sa, &tmA1, &full_bar[stage], (rem - g.kb0) * BK, x0 + dx, y0 + dy, n0);
-              kcoord = tap_k + g.c0 + (rem - g.kb0) * BK;
+              tma_load_4d(sa, &tmA1, &full_bar[stage], (rem - g.kb0) * kConvKel, x0 + dx, y0 + dy, n0);
+              kcoord = tap_k + g.c0 + (rem - g.kb0) * kConvKel;
             }
             tma_load_2d(sb, &tmB, &full_bar[stage], kcoord, n_tile * BN);
           }
@@ -209,8 +214,14 @@
         float* sas = sbias + 1024 + (lt & 1u) * 128;
         const int col = n_tile * BN + ct;
         if (ct < BN) sws[ct] = col < N ? __ldg(w_scale + col) : 0.f;
-        const int r = m_tile * BM + ct;
-        if (ct < BM) sas[ct] = r < M ? __ldg(a_scale + r) : 0.f;
+        if constexpr (kImgScale) {
+          // conv: one scale per image; tile row ct lies in image n0 + ct / (TW TH) of the {TW, TH, TN} footprint
+          const int img = n0 + ct / (g.TW * g.TH);
+          if (ct < BM) sas[ct] = img < g.NI ? __ldg(a_scale + img) : 0.f;
+        } else {
+          const int r = m_tile * BM + ct;
+          if (ct < BM) sas[ct] = r < M ? __ldg(a_scale + r) : 0.f;
+        }
       }
 
       // ---- main loop: one wgmma group per k-block; the stage of k-block i - 1 is released once group i is issued ----

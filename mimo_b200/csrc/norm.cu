@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdio.h>
 
+#include <type_traits>
+
 #include "../../include/mimo_b200.h"
 #include "host_util.h"
 #include "ptx.cuh"
@@ -42,6 +44,15 @@ struct GnArgs {
   const float* stats;  // [samples][groups][2] = (mean, rstd)
 };
 
+// the e4m3 output (mimo_groupnorm_e4m3; out is one byte per element). A separate type, so that the 16-bit kernels keep
+// their parameter block.
+struct GnE4m3Args : GnArgs {
+  float* mm;      // [n][bpi][groups][2] = (min, max) of x per slab; per image, also in window mode (never gathered)
+  float* qscale;  // [n]: the image's scale amax / 448
+};
+template <bool kE4m3>
+using GnArgsT = std::conditional_t<kE4m3, GnE4m3Args, GnArgs>;
+
 template <bool kBf16>
 __device__ __forceinline__ uint4 gn_load(const GnArgs& a, long long pix, int cv) {
   using C = Cvt<kBf16>;
@@ -68,10 +79,11 @@ constexpr int kGnMaxThreads = 320;
 
 // pass 1: per-(image, slab, group) sum and sum of squares. kWindow: the image is frame k of sample s, and the block
 // writes slab row 1 + blockIdx.x of record (k, s); the first slab's block also writes the record's K_g row.
-template <bool kBf16, bool kWindow = false>
-__global__ void __launch_bounds__(kGnMaxThreads) gn_stats_kernel(GnArgs a) {
+// kMinMax (the e4m3 output): also the slab's per-group min / max of x, into a.mm (per image, outside the window table).
+template <bool kBf16, bool kWindow = false, bool kMinMax = false>
+__global__ void __launch_bounds__(kGnMaxThreads) gn_stats_kernel(GnArgsT<kMinMax> a) {
   using C = Cvt<kBf16>;
-  __shared__ float4 s_red[kGnMaxThreads];  // per-thread (sumA, sqA, sumB, sqB)
+  __shared__ float4 s_red[kGnMaxThreads];  // per-thread (sumA, sqA, sumB, sqB); with kMinMax then (loA, hiA, loB, hiB)
   pdl_launch_dependents();
   pdl_wait();
   const int n = blockIdx.y;
@@ -84,6 +96,7 @@ __global__ void __launch_bounds__(kGnMaxThreads) gn_stats_kernel(GnArgs a) {
   int split = (gA + 1) * a.cpg - ch0;  // channels [0, split) of this vector belong to gA, the rest to gA + 1
   if (split > 8) split = 8;
   float sA = 0.f, qA = 0.f, sB = 0.f, qB = 0.f;
+  [[maybe_unused]] float lA = INFINITY, hA = -INFINITY, lB = INFINITY, hB = -INFINITY;
   if (active) {
     const float kA = gn_shift<kBf16>(a, n, gA), kB = split < 8 ? gn_shift<kBf16>(a, n, gA + 1) : 0.f;
     const int p_begin = blockIdx.x * a.pix_per_block;
@@ -109,6 +122,12 @@ __global__ void __launch_bounds__(kGnMaxThreads) gn_stats_kernel(GnArgs a) {
         } else {
           const float d = t.y - kB;
           sB += d, qB += d * d;
+        }
+        if constexpr (kMinMax) {
+          if (2 * j < split) lA = fminf(lA, t.x), hA = fmaxf(hA, t.x);
+          else lB = fminf(lB, t.x), hB = fmaxf(hB, t.x);
+          if (2 * j + 1 < split) lA = fminf(lA, t.y), hA = fmaxf(hA, t.y);
+          else lB = fminf(lB, t.y), hB = fmaxf(hB, t.y);
         }
       }
     }
@@ -143,11 +162,84 @@ __global__ void __launch_bounds__(kGnMaxThreads) gn_stats_kernel(GnArgs a) {
       dst[1] = q;
     }
   }
+  if constexpr (kMinMax) {
+    __syncthreads();
+    s_red[tid] = make_float4(lA, hA, lB, hB);
+    __syncthreads();
+    for (int g = tid; g < a.groups; g += blockDim.x) {
+      const int v_lo = (g * a.cpg) >> 3;
+      const int v_hi = ((g + 1) * a.cpg - 1) >> 3;
+      float lo = INFINITY, hi = -INFINITY;
+      for (int v = v_lo; v <= v_hi; ++v) {
+        const bool as_a = (v * 8) / a.cpg == g;
+        for (int l = 0; l < a.P; ++l) {
+          const float4 r = s_red[l * a.vecs + v];
+          lo = fminf(lo, as_a ? r.x : r.z);
+          hi = fmaxf(hi, as_a ? r.y : r.w);
+        }
+      }
+      float* dst = a.mm + ((static_cast<long long>(n) * a.bpi + blockIdx.x) * a.groups + g) * 2;
+      dst[0] = lo;
+      dst[1] = hi;
+    }
+  }
 }
 
-// normalise + affine (+ SiLU) of image n's slab blockIdx.x, with the per-group mean / rstd in shared memory
+// SiLU's only turning point: its minimum silu(-1.2784645) = -0.27846454
+constexpr float kSiluArgMin = -1.2784645f;
+constexpr float kSiluMinAbs = 0.27846454f;
+
+// e4m3 output: the image's bound amax on |SiLU(GroupNorm(x))| (include/mimo_b200.h, mimo_groupnorm_e4m3), from the slab
+// min / max of pass 1 and the normaliser's mean / rstd. Every block of the image computes the same value (min / max are
+// exact in any order); the first writes the scale. Returns 448 / amax (1 for a zero bound) to every thread.
 template <bool kBf16>
-__device__ __forceinline__ void gn_normalise(const GnArgs& a, int n, const float* s_mean, const float* s_rstd) {
+__device__ float gn_e4m3_inv(const GnE4m3Args& a, int n, const float* s_mean, const float* s_rstd) {
+  using C = Cvt<kBf16>;
+  using T = typename C::T;
+  __shared__ float s_lo[64], s_hi[64], s_wmax[kGnMaxThreads / 32], s_inv;
+  const int tid = threadIdx.x;
+  const long long g2 = 2LL * a.groups;
+  for (int g = tid; g < a.groups; g += blockDim.x) {
+    const float* src = a.mm + static_cast<long long>(n) * a.bpi * g2 + 2 * g;
+    float lo = INFINITY, hi = -INFINITY;
+    for (int b = 0; b < a.bpi; ++b) {
+      lo = fminf(lo, src[b * g2]);
+      hi = fmaxf(hi, src[b * g2 + 1]);
+    }
+    s_lo[g] = lo;
+    s_hi[g] = hi;
+  }
+  __syncthreads();
+  float m = 0.f;
+  for (int c = tid; c < a.C; c += blockDim.x) {
+    const int g = c / a.cpg;
+    // the same products as gn_normalise: y = fmaf(x - mean, rstd * gamma, beta)
+    const float sc = s_rstd[g] * C::to_f(static_cast<const T*>(a.gamma)[c]);
+    const float bc = C::to_f(static_cast<const T*>(a.beta)[c]);
+    const float zl = fmaf(s_lo[g] - s_mean[g], sc, bc), zh = fmaf(s_hi[g] - s_mean[g], sc, bc);
+    float bnd = fmaxf(fabsf(silu_f(zl)), fabsf(silu_f(zh)));
+    if (fminf(zl, zh) <= kSiluArgMin && fmaxf(zl, zh) >= kSiluArgMin) bnd = fmaxf(bnd, kSiluMinAbs);
+    m = fmaxf(m, bnd);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((tid & 31) == 0) s_wmax[tid >> 5] = m;
+  __syncthreads();
+  if (tid == 0) {
+    float amax = 0.f;
+    for (int w = 0; w < static_cast<int>(blockDim.x >> 5); ++w) amax = fmaxf(amax, s_wmax[w]);
+    s_inv = amax == 0.f ? 1.f : 448.0f / amax;
+    if (blockIdx.x == 0) a.qscale[n] = amax == 0.f ? 1.f : amax / 448.0f;
+  }
+  __syncthreads();
+  return s_inv;
+}
+
+// normalise + affine (+ SiLU) of image n's slab blockIdx.x, with the per-group mean / rstd in shared memory.
+// kE4m3: always SiLU, then cvt.rn.satfinite.e4m3(y * inv) into one-byte elements.
+template <bool kBf16, bool kE4m3 = false>
+__device__ __forceinline__ void gn_normalise(const GnArgs& a, int n, const float* s_mean, const float* s_rstd,
+                                             [[maybe_unused]] float inv = 1.f) {
   using C = Cvt<kBf16>;
   const int tid = threadIdx.x;
   const int cv = tid % a.vecs;
@@ -196,22 +288,34 @@ __device__ __forceinline__ void gn_normalise(const GnArgs& a, int n, const float
       f[2 * j] = fmaf(t.x - (2 * j < split ? mA : mB), sc[2 * j], bc[2 * j]);
       f[2 * j + 1] = fmaf(t.y - (2 * j + 1 < split ? mA : mB), sc[2 * j + 1], bc[2 * j + 1]);
     }
-    if (a.silu) {
+    if constexpr (kE4m3) {
+      uint32_t q[2];  // elements 4 j .. 4 j + 3 in q[j], lowest address in the lowest byte
 #pragma unroll
-      for (int j = 0; j < 8; ++j) f[j] = silu_f(f[j]);
+      for (int j = 0; j < 2; ++j) {
+        uint16_t lo, hi;  // cvt packs its first source into the upper byte
+        asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(lo) : "f"(silu_f(f[4 * j + 1]) * inv), "f"(silu_f(f[4 * j]) * inv));
+        asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(hi) : "f"(silu_f(f[4 * j + 3]) * inv), "f"(silu_f(f[4 * j + 2]) * inv));
+        q[j] = static_cast<uint32_t>(lo) | (static_cast<uint32_t>(hi) << 16);
+      }
+      *reinterpret_cast<uint2*>(static_cast<uint8_t*>(a.out) + pix * a.C + ch0) = make_uint2(q[0], q[1]);
+    } else {
+      if (a.silu) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) f[j] = silu_f(f[j]);
+      }
+      uint4 o;
+      o.x = C::pack(f[0], f[1]);
+      o.y = C::pack(f[2], f[3]);
+      o.z = C::pack(f[4], f[5]);
+      o.w = C::pack(f[6], f[7]);
+      *reinterpret_cast<uint4*>(static_cast<typename C::T*>(a.out) + pix * a.C + ch0) = o;
     }
-    uint4 o;
-    o.x = C::pack(f[0], f[1]);
-    o.y = C::pack(f[2], f[3]);
-    o.z = C::pack(f[4], f[5]);
-    o.w = C::pack(f[6], f[7]);
-    *reinterpret_cast<uint4*>(static_cast<typename C::T*>(a.out) + pix * a.C + ch0) = o;
   }
 }
 
-// pass 2: image statistics from the slab partials (fixed order), then normalise + affine (+ SiLU)
-template <bool kBf16>
-__global__ void __launch_bounds__(kGnMaxThreads) gn_apply_kernel(GnArgs a) {
+// pass 2: image statistics from the slab partials (fixed order), then normalise + affine (+ SiLU) (kE4m3: -> e4m3)
+template <bool kBf16, bool kE4m3 = false>
+__global__ void __launch_bounds__(kGnMaxThreads) gn_apply_kernel(GnArgsT<kE4m3> a) {
   __shared__ float s_tot[4][128];
   __shared__ float s_mean[64], s_rstd[64];
   pdl_launch_dependents();
@@ -246,7 +350,10 @@ __global__ void __launch_bounds__(kGnMaxThreads) gn_apply_kernel(GnArgs a) {
     }
     __syncthreads();
   }
-  gn_normalise<kBf16>(a, n, s_mean, s_rstd);
+  if constexpr (kE4m3)
+    gn_normalise<kBf16, true>(a, n, s_mean, s_rstd, gn_e4m3_inv<kBf16>(a, n, s_mean, s_rstd));
+  else
+    gn_normalise<kBf16>(a, n, s_mean, s_rstd);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -306,8 +413,8 @@ __global__ void __launch_bounds__(kGnwReduceThreads) gnw_reduce_kernel(GnArgs a,
   }
 }
 
-template <bool kBf16>
-__global__ void __launch_bounds__(kGnMaxThreads) gnw_apply_kernel(GnArgs a) {
+template <bool kBf16, bool kE4m3 = false>
+__global__ void __launch_bounds__(kGnMaxThreads) gnw_apply_kernel(GnArgsT<kE4m3> a) {
   __shared__ float s_mean[64], s_rstd[64];
   pdl_launch_dependents();
   pdl_wait();
@@ -318,7 +425,10 @@ __global__ void __launch_bounds__(kGnMaxThreads) gnw_apply_kernel(GnArgs a) {
     s_rstd[g] = st[2 * g + 1];
   }
   __syncthreads();
-  gn_normalise<kBf16>(a, n, s_mean, s_rstd);
+  if constexpr (kE4m3)  // the window's mean / rstd with this frame's own min / max
+    gn_normalise<kBf16, true>(a, n, s_mean, s_rstd, gn_e4m3_inv<kBf16>(a, n, s_mean, s_rstd));
+  else
+    gn_normalise<kBf16>(a, n, s_mean, s_rstd);
 }
 
 // launch geometry shared by mimo_groupnorm and mimo_groupnorm_workspace_bytes
@@ -692,7 +802,7 @@ extern "C" int mimo_groupnorm(const mimo_groupnorm_params* p, void* stream) {
     return set_error(MIMO_ERR_ARG, "mimo_groupnorm: null pointer");
   if (int rc = ensure_device()) return rc;
   const GnPlan pl = gn_plan(p->n, p->hw, C);
-  GnArgs a;
+  GnArgs a = {};
   a.x0 = p->x0;
   a.x1 = p->x1;
   a.gamma = p->gamma;
@@ -754,7 +864,7 @@ static long long gnw_rec_floats(const GnPlan& pl, int groups) {
 }
 
 static GnArgs gnw_args(const mimo_groupnorm_window_params* p, int C, const GnPlan& pl) {
-  GnArgs a;
+  GnArgs a = {};
   a.x0 = p->x0;
   a.x1 = p->x1;
   a.gamma = p->gamma;
@@ -850,6 +960,106 @@ extern "C" int mimo_groupnorm_window_apply(const mimo_groupnorm_window_params* p
     return set_error(MIMO_ERR_ARG, "mimo_groupnorm_window_apply: partial table smaller than table_frames records");
   if (int rc = ensure_device()) return rc;
   return gnw_launch(p, C, false, true, p->table_frames, stream);
+}
+
+// ---- GroupNorm + SiLU -> e4m3 ----
+static mimo_groupnorm_window_params gn8_as_window(const mimo_groupnorm_e4m3_params* p) {
+  mimo_groupnorm_window_params w = {};
+  w.x0 = p->x0;
+  w.c0 = p->c0;
+  w.x1 = p->x1;
+  w.c1 = p->c1;
+  w.gamma = p->gamma;
+  w.beta = p->beta;
+  w.out = p->out;
+  w.table = p->table;
+  w.table_bytes = p->table_bytes;
+  w.samples = p->samples;
+  w.frames = p->frames;
+  w.table_frames = p->table_frames;
+  w.hw = p->hw;
+  w.groups = p->groups;
+  w.eps = p->eps;
+  w.silu = 1;
+  w.dtype = p->dtype;
+  return w;
+}
+
+// work: [images][bpi][groups][2] (min, max) of x, then the per-image partials ([images][bpi][groups][2], FRAME mode) or
+// the window statistics ([samples][groups][2], window modes)
+static int gn8_sizes(const mimo_groupnorm_e4m3_params* p, int* C, GnPlan* pl, long long* mm_floats, int64_t* work_bytes) {
+  if (!p) return set_error(MIMO_ERR_ARG, "mimo_groupnorm_e4m3: null params");
+  if (p->mode < MIMO_GN_E4M3_FRAME || p->mode > MIMO_GN_E4M3_WINDOW_APPLY)
+    return set_error(MIMO_ERR_ARG, "mimo_groupnorm_e4m3: unknown mode");
+  const mimo_groupnorm_window_params w = gn8_as_window(p);
+  if (int rc = gnw_check(&w, "mimo_groupnorm_e4m3", C)) return rc;
+  *pl = gn_plan(p->samples * p->frames, p->hw, *C);
+  *mm_floats = static_cast<long long>(p->samples) * p->frames * pl->bpi * p->groups * 2;
+  const long long rest = p->mode == MIMO_GN_E4M3_FRAME ? *mm_floats : 2LL * p->samples * p->groups;
+  *work_bytes = static_cast<int64_t>((*mm_floats + rest) * sizeof(float));
+  return MIMO_OK;
+}
+
+extern "C" int64_t mimo_groupnorm_e4m3_workspace_bytes(const mimo_groupnorm_e4m3_params* p) {
+  int C = 0;
+  GnPlan pl;
+  long long mmf = 0;
+  int64_t wb = 0;
+  if (int rc = gn8_sizes(p, &C, &pl, &mmf, &wb)) return rc;
+  return wb;
+}
+
+extern "C" int mimo_groupnorm_e4m3(const mimo_groupnorm_e4m3_params* p, void* stream) {
+  int C = 0;
+  GnPlan pl;
+  long long mmf = 0;
+  int64_t wb = 0;
+  if (int rc = gn8_sizes(p, &C, &pl, &mmf, &wb)) return rc;
+  const int mode = p->mode;
+  const bool window = mode != MIMO_GN_E4M3_FRAME;
+  const bool partials = mode != MIMO_GN_E4M3_WINDOW_APPLY, apply = mode != MIMO_GN_E4M3_WINDOW_PARTIALS;
+  if (!p->x0 || !p->work || (apply && (!p->gamma || !p->beta || !p->out || !p->scale)) || (window && !p->table))
+    return set_error(MIMO_ERR_ARG, "mimo_groupnorm_e4m3: null pointer");
+  if (p->work_bytes < wb) return set_error(MIMO_ERR_ARG, "mimo_groupnorm_e4m3: work smaller than its workspace bytes");
+  if (mode == MIMO_GN_E4M3_WINDOW_APPLY && p->table_frames < p->frames)
+    return set_error(MIMO_ERR_ARG, "mimo_groupnorm_e4m3: table_frames must be >= frames (the whole window)");
+  const mimo_groupnorm_window_params w = gn8_as_window(p);
+  const int table_frames = mode == MIMO_GN_E4M3_WINDOW_APPLY ? p->table_frames : p->frames;
+  if (window && p->table_bytes < gnw_table_bytes(&w, C, table_frames))
+    return set_error(MIMO_ERR_ARG, "mimo_groupnorm_e4m3: partial table smaller than its records");
+  if (int rc = ensure_device()) return rc;
+  GnE4m3Args a;
+  static_cast<GnArgs&>(a) = gnw_args(&w, C, pl);
+  a.mm = p->work;
+  a.qscale = p->scale;
+  float* rest = p->work + mmf;
+  if (!window) a.part = rest;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const dim3 grid(pl.bpi, p->samples * p->frames);
+  const bool bf = p->dtype == MIMO_BF16;
+  cudaError_t e = cudaSuccess;
+  if (!window) {
+    e = bf ? launch_k(gn_stats_kernel<true, false, true>, grid, dim3(pl.threads), 0, st, a)
+           : launch_k(gn_stats_kernel<false, false, true>, grid, dim3(pl.threads), 0, st, a);
+    if (e == cudaSuccess)
+      e = bf ? launch_k(gn_apply_kernel<true, true>, grid, dim3(pl.threads), 0, st, a)
+             : launch_k(gn_apply_kernel<false, true>, grid, dim3(pl.threads), 0, st, a);
+  } else {
+    if (partials)
+      e = bf ? launch_k(gn_stats_kernel<true, true, true>, grid, dim3(pl.threads), 0, st, a)
+             : launch_k(gn_stats_kernel<false, true, true>, grid, dim3(pl.threads), 0, st, a);
+    if (apply && e == cudaSuccess) {
+      a.stats = rest;
+      e = launch_k(gnw_reduce_kernel, dim3(p->samples), dim3(kGnwReduceThreads), 0, st, static_cast<const GnArgs&>(a),
+                   table_frames, rest);
+      if (e == cudaSuccess)
+        e = bf ? launch_k(gnw_apply_kernel<true, true>, grid, dim3(pl.threads), 0, st, a)
+               : launch_k(gnw_apply_kernel<false, true>, grid, dim3(pl.threads), 0, st, a);
+    }
+  }
+  if (e == cudaSuccess) e = cudaGetLastError();
+  if (e != cudaSuccess) return set_cuda_error("groupnorm_e4m3 launch", e);
+  return MIMO_OK;
 }
 
 extern "C" int mimo_layernorm(const void* x, const void* gamma, const void* beta, void* out, int64_t rows,

@@ -150,6 +150,9 @@ class UNetEngine:
         self.fp8 = False
         self.w8: Optional[Dict[str, dict]] = None
         self._cache8: Optional[Path] = None  # file of the e4m3 copies in the weight cache (when one is set)
+        # set_fp8(True, convs=True): e4m3 copies of every ResnetBlock3D conv1 / conv2, in their own cache file
+        self.w8c: Optional[Dict[str, dict]] = None
+        self._cache8c: Optional[Path] = None
         # packed weights: from the on-disk cache when MIMO_B200_WEIGHT_CACHE is set and holds this state dict
         from .host import weight_cache as WC
         cache = WC.cache_dir()
@@ -159,6 +162,7 @@ class UNetEngine:
             cfile = cache / f"unet-{key}.safetensors"
             # the e4m3 copies are a function of the packed weights, which `key` already identifies: no second pass over sd
             self._cache8 = cache / f"unet-e4m3-{WC.fingerprint({}, extra=f'unet-e4m3|{key}')}.safetensors"
+            self._cache8c = cache / f"unet-e4m3conv-{WC.fingerprint({}, extra=f'unet-e4m3conv|{key}')}.safetensors"
             if cfile.exists():
                 st = WC.load(cfile, self.device)
                 self.w, self.resnets, self.xf_paths = st["w"], st["resnets"], st["xf_paths"]
@@ -284,29 +288,45 @@ class UNetEngine:
                     w8[f"{p}.{k}"] = {"qkv": [q(a["qkv"]) for a in blk["attn"]], "geglu": q(blk["geglu"][0])}
         return w8
 
-    def set_fp8(self, on: bool) -> None:
-        """Run the LN-fed projections (see _pack_e4m3) as LayerNorm -> e4m3 rows + scales -> e4m3 GEMM. Captured graphs
+    def _pack_e4m3_convs(self) -> Dict[str, dict]:
+        """e4m3 copies (one fp32 scale per output channel) of every ResnetBlock3D's conv1 and conv2 [Cout, 9 Cin] packs"""
+        q = ops.pack_e4m3_weight
+        return {p: {"c1": q(self.w[p]["c1"][0]), "c2": q(self.w[p]["c2"][0])} for p in self.resnets}
+
+    def _e4m3_copies(self, cfile: Optional[Path], pack) -> Dict[str, dict]:
+        from .host import weight_cache as WC
+        if cfile is not None and cfile.exists():
+            return WC.load(cfile, self.device)
+        w8 = pack()
+        if cfile is not None:
+            WC.save(cfile, w8)
+        return w8
+
+    def set_fp8(self, on: bool, convs: bool = False) -> None:
+        """Run the LN-fed projections (see _pack_e4m3) as LayerNorm -> e4m3 rows + scales -> e4m3 GEMM; with `convs`, also
+        every ResnetBlock3D conv1 / conv2 as GroupNorm + SiLU -> e4m3 + one scale per image -> e4m3 conv. Captured graphs
         are dropped whenever the setting changes."""
-        on = bool(on)
-        if on == self.fp8:
+        on, convs = bool(on), bool(convs)
+        if convs and not on:
+            raise ValueError("set_fp8(False, convs=True): the FP8 convolutions come on top of the FP8 projections")
+        if on == self.fp8 and convs == self.fp8_convs:
             return
         if on and self.w8 is None:
-            from .host import weight_cache as WC
-            cfile = self._cache8
-            if cfile is not None and cfile.exists():
-                self.w8 = WC.load(cfile, self.device)
-            else:
-                self.w8 = self._pack_e4m3()
-                if cfile is not None:
-                    WC.save(cfile, self.w8)
-        self.fp8 = on
+            self.w8 = self._e4m3_copies(self._cache8, self._pack_e4m3)
+        if convs and self.w8c is None:
+            self.w8c = self._e4m3_copies(self._cache8c, self._pack_e4m3_convs)
+        self.fp8, self.fp8_convs = on, convs
         self._graphs.clear()
 
     def fp8_bytes(self) -> int:
-        """device bytes of the e4m3 copies (0 before the first set_fp8(True))"""
+        """device bytes of the e4m3 copies (0 before the first set_fp8(True)): the projections' and, once the convs were
+        turned on, the convs'"""
         out = 0
         for m in (self.w8 or {}).values():
             for wq, ws in [m["geglu"]] + (m["qkv"] if isinstance(m["qkv"], list) else [m["qkv"]]):
+                out += wq.numel() * wq.element_size() + ws.numel() * ws.element_size()
+        for m in (self.w8c or {}).values():
+            for wq, ws in m.values():
                 out += wq.numel() * wq.element_size() + ws.numel() * ws.element_size()
         return out
 
@@ -332,48 +352,68 @@ class UNetEngine:
     def _time_embed(self, timesteps: torch.Tensor) -> torch.Tensor:
         return self._time_embed_from(self._sinusoid(timesteps))
 
-    def _norm_silu(self, x0, gb, n, hw, rows_per_branch, window: bool, slot: str, x1=None):
+    def _norm_silu(self, x0, gb, n, hw, rows_per_branch, window: bool, slot: str, x1=None, e4m3=False):
         """SiLU(GroupNorm) of a ResnetBlock3D or of conv_norm_out (eps = norm_eps). Per frame, or with `window` over
         all frames of each CFG branch (rows_per_branch = frames * hw). Frame-sharded (self.xchg, G GPUs): every member
         writes the partial table of its frames into its peer buffer `slot`, the group all-gathers the tables (bytes
-        moved as they are) and every member normalises its frames from the whole window's table."""
+        moved as they are) and every member normalises its frames from the whole window's table.
+        `e4m3`: returns (e4m3 output, one scale per frame) for conv3x3_e4m3 instead; the per-frame min / max the scales
+        are built from stay on this GPU, so the exchange is the same."""
         g, eps = self.spec.norm_num_groups, self.spec.norm_eps
         if not window:
+            if e4m3:
+                return ops.groupnorm_e4m3(x0, *gb, n, hw, groups=g, eps=eps, x1=x1)
             return ops.groupnorm(x0, *gb, n, hw, groups=g, eps=eps, silu=True, x1=x1)
         f = rows_per_branch // hw
         b = n // f
         xg = self.xchg
         if xg is None or xg.G == 1:
+            if e4m3:
+                return ops.groupnorm_e4m3(x0, *gb, n, hw, groups=g, eps=eps, x1=x1, window_frames=f)
             return ops.groupnorm_window(x0, *gb, b, f, hw, groups=g, eps=eps, silu=True, x1=x1)
         c = x0.shape[1] + (x1.shape[1] if x1 is not None else 0)
         need = ops.groupnorm_window_table_bytes(b, f, hw, c, g)
         if slot not in xg.bufs or xg.bufs[slot].nbytes < need:
             raise L.MimoError(f"frame-sharded window GroupNorm needs a peer buffer '{slot}' of {need} bytes")
         mine = xg.bufs[slot].bytes[:need].view(torch.float32)
-        ops.groupnorm_window_partials(x0, b, f, hw, groups=g, x1=x1, table=mine)
+        if e4m3:
+            _, work = ops.groupnorm_e4m3_partials(x0, b, f, hw, groups=g, x1=x1, table=mine)
+        else:
+            ops.groupnorm_window_partials(x0, b, f, hw, groups=g, x1=x1, table=mine)
         table = torch.empty((xg.G * need // 4,), dtype=torch.float32, device=x0.device)
         xg.pull(2, slot, table.view(torch.float16).view(-1, 8), 1, 1, need // 16, 8)  # fp32 bytes as 16-bit pairs
+        if e4m3:
+            return ops.groupnorm_e4m3_apply(x0, *gb, table, work, b, f, f * xg.G, hw, groups=g, eps=eps, x1=x1)
         return ops.groupnorm_window_apply(x0, *gb, table, b, f, f * xg.G, hw, groups=g, eps=eps, silu=True, x1=x1)
 
     _window_gn = False  # whether the forward being recorded runs the ResBlocks' GroupNorms over the window (_forward_impl)
+    fp8_convs = False  # whether the ResBlock convs run from e4m3 operands (set_fp8)
 
     def _resnet(self, p, x0, x1, tembs, n, h, w, rows_per_branch):
         r = self.w[p]
         hw = h * w
         window_gn = self._window_gn
+        w8 = self.w8c[p] if self.fp8_convs else None
+
         # window mode, frame-sharded: norm1 and norm2 gather through two peer buffers used alternately, so a member only
         # rewrites one after the exchange in between (csrc/exchange.cu); the output norm has a third
-        t = self._norm_silu(x0, r["n1"], n, hw, rows_per_branch, window_gn, "N0", x1=x1)
+        def norm(x, xx1, key, slot):  # FP8 convs: (e4m3 output, one scale per frame)
+            return self._norm_silu(x, r[key], n, hw, rows_per_branch, window_gn, slot, x1=xx1, e4m3=w8 is not None)
+
+        def conv(t, key, **ep):
+            if w8 is None:
+                return ops.conv3x3(t, r[key][0], n, h, w, bias=r[key][1], **ep)
+            return ops.conv3x3_e4m3(*t, *w8[key], n, h, w, x0.dtype, bias=r[key][1], **ep)
+
         off, cout = self.temb_off[p]
-        t = ops.conv3x3(t, r["c1"][0], n, h, w, bias=r["c1"][1], rowvec=tembs[:, off:off + cout],
-                        rows_per_group=rows_per_branch)
-        t = self._norm_silu(t, r["n2"], n, hw, rows_per_branch, window_gn, "N1")
+        t = conv(norm(x0, x1, "n1", "N0"), "c1", rowvec=tembs[:, off:off + cout], rows_per_group=rows_per_branch)
+        t = norm(t, None, "n2", "N1")
         if r["sc"] is not None:
             res = ops.gemm(x0, r["sc"][0], a1=x1, bias=r["sc"][1])
         else:
             assert x1 is None
             res = x0
-        return ops.conv3x3(t, r["c2"][0], n, h, w, bias=r["c2"][1], residual=res)
+        return conv(t, "c2", residual=res)
 
     def _ff(self, x, ln, geglu, ffo, geglu8=None):
         if geglu8 is None:

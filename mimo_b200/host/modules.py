@@ -316,21 +316,25 @@ class UNet3DConditionModel(_UNetBase):
         self._spec.inflated_groupnorm = self.use_inflated_groupnorm
 
     _fp8 = False
+    _fp8_convs = False
 
-    def enable_fp8(self):
+    def enable_fp8(self, convs: bool = False):
         """Run the q|k|v and GEGLU projections that read a LayerNorm output in FP8 (e4m3 activations with one scale per
-        token, e4m3 weights with one scale per output channel, fp32 accumulation). Everything else stays in the model
-        dtype. The e4m3 weight copies are made on first use and kept; captured CUDA graphs of the forward are dropped."""
+        token, e4m3 weights with one scale per output channel, fp32 accumulation). With `convs`, every ResnetBlock3D
+        conv1 / conv2 also runs from e4m3 operands: its GroupNorm + SiLU writes e4m3 with one scale per frame, the weights
+        have one scale per output channel. Everything else stays in the model dtype. The e4m3 weight copies are made on
+        first use and kept; captured CUDA graphs of the forward are dropped."""
         if self.dtype not in (torch.float16, torch.bfloat16):
             raise MimoError(f"enable_fp8() needs an fp16 or bf16 model, not {self.dtype}")
-        self._fp8 = True
+        self._fp8, self._fp8_convs = True, bool(convs)
         if self._engine is not None:
-            self._engine.set_fp8(True)
+            self._engine.set_fp8(True, convs=self._fp8_convs)
         return self
 
     def disable_fp8(self):
-        """Back to the model dtype for every projection (the e4m3 copies stay packed for a later enable_fp8())."""
-        self._fp8 = False
+        """Back to the model dtype for every projection and conv (the e4m3 copies stay packed for a later
+        enable_fp8())."""
+        self._fp8 = self._fp8_convs = False
         if self._engine is not None:
             self._engine.set_fp8(False)
         return self
@@ -339,9 +343,13 @@ class UNet3DConditionModel(_UNetBase):
     def fp8_enabled(self) -> bool:
         return self._fp8
 
+    @property
+    def fp8_convs_enabled(self) -> bool:
+        return self._fp8_convs
+
     def engine(self) -> E.UNetEngine:
         eng = super().engine()
-        eng.set_fp8(self._fp8)
+        eng.set_fp8(self._fp8, convs=self._fp8_convs)
         return eng
 
     @classmethod

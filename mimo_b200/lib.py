@@ -101,6 +101,38 @@ class GroupNormWindowParams(C.Structure):
     ]
 
 
+GN_E4M3_FRAME, GN_E4M3_WINDOW, GN_E4M3_WINDOW_PARTIALS, GN_E4M3_WINDOW_APPLY = 0, 1, 2, 3
+
+
+class GroupNormE4m3Params(C.Structure):
+    _fields_ = [
+        ("x0", C.c_void_p), ("c0", C.c_int32),
+        ("x1", C.c_void_p), ("c1", C.c_int32),
+        ("gamma", C.c_void_p), ("beta", C.c_void_p),
+        ("out", C.c_void_p),
+        ("scale", C.c_void_p),
+        ("work", C.c_void_p), ("work_bytes", C.c_int64),
+        ("table", C.c_void_p), ("table_bytes", C.c_int64),
+        ("mode", C.c_int32),
+        ("samples", C.c_int32), ("frames", C.c_int32), ("table_frames", C.c_int32), ("hw", C.c_int32),
+        ("groups", C.c_int32),
+        ("eps", C.c_float),
+        ("dtype", C.c_int32),
+    ]
+
+
+class Conv3x3E4m3Params(C.Structure):
+    _fields_ = [
+        ("x", C.c_void_p), ("x_scale", C.c_void_p), ("c_in", C.c_int32),
+        ("w", C.c_void_p), ("w_scale", C.c_void_p),
+        ("out", C.c_void_p), ("ldo", C.c_int64),
+        ("n", C.c_int32), ("h", C.c_int32), ("w_", C.c_int32), ("cout", C.c_int32),
+        ("dtype", C.c_int32),
+        ("ep", Epilogue),
+        ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64),
+    ]
+
+
 class AttnParams(C.Structure):
     _fields_ = [
         ("q", C.c_void_p), ("k", C.c_void_p), ("v", C.c_void_p), ("ld_qkv", C.c_int64),
@@ -163,6 +195,7 @@ SYMBOLS = {
     "mimo_gemm_e4m3": (C.c_int, [C.POINTER(GemmE4m3Params), _VP]),
     "mimo_conv3x3": (C.c_int, [C.POINTER(Conv3x3Params), _VP]),
     "mimo_conv_up2x": (C.c_int, [C.POINTER(Conv3x3Params), _VP]),
+    "mimo_conv3x3_e4m3": (C.c_int, [C.POINTER(Conv3x3E4m3Params), _VP]),
     "mimo_im2col3x3": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I64, _I32, _VP]),
     "mimo_groupnorm": (C.c_int, [C.POINTER(GroupNormParams), _VP]),
     "mimo_groupnorm_workspace_bytes": (C.c_int64, [C.POINTER(GroupNormParams)]),
@@ -170,6 +203,8 @@ SYMBOLS = {
     "mimo_groupnorm_window_partials": (C.c_int, [C.POINTER(GroupNormWindowParams), _VP]),
     "mimo_groupnorm_window_apply": (C.c_int, [C.POINTER(GroupNormWindowParams), _VP]),
     "mimo_groupnorm_window_table_bytes": (C.c_int64, [C.POINTER(GroupNormWindowParams)]),
+    "mimo_groupnorm_e4m3": (C.c_int, [C.POINTER(GroupNormE4m3Params), _VP]),
+    "mimo_groupnorm_e4m3_workspace_bytes": (C.c_int64, [C.POINTER(GroupNormE4m3Params)]),
     "mimo_layernorm": (C.c_int, [_VP, _VP, _VP, _VP, _I64, _I32, _F, _VP, _I64, _I32, _I32, _I32, _VP]),
     "mimo_layernorm_e4m3": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _I64, _I32, _F, _VP, _I64, _I32, _I32, _I32, _VP]),
     "mimo_attn_spatial": (C.c_int, [C.POINTER(AttnParams), _VP]),
@@ -216,7 +251,8 @@ def load() -> C.CDLL:
         fn.restype = res
         fn.argtypes = args
     for which, st in enumerate((Epilogue, GemmParams, Conv3x3Params, GroupNormParams, AttnParams, AttnTemporalParams,
-                             ExchangeParams, CfgMultistepParams, GroupNormWindowParams, GemmE4m3Params)):
+                             ExchangeParams, CfgMultistepParams, GroupNormWindowParams, GemmE4m3Params,
+                             GroupNormE4m3Params, Conv3x3E4m3Params)):
         if lib.mimo_abi_sizeof(which) != C.sizeof(st):
             raise MimoError(f"ABI mismatch: {st.__name__} is {C.sizeof(st)} bytes in lib.py but "
                             f"{lib.mimo_abi_sizeof(which)} in {LIB_PATH.name}; rebuild the library")

@@ -183,6 +183,34 @@ def conv3x3(x0: torch.Tensor, w: torch.Tensor, n: int, h: int, wd: int, out: Opt
     return out
 
 
+def conv3x3_e4m3(x: torch.Tensor, x_scale: torch.Tensor, w: torch.Tensor, w_scale: torch.Tensor, n: int, h: int,
+                 wd: int, dtype: torch.dtype, out: Optional[torch.Tensor] = None, *, bias=None, rowvec=None,
+                 rows_per_group: Optional[int] = None, residual=None, scale=1.0, act=L.ACT_NONE) -> torch.Tensor:
+    """conv3x3() from e4m3 operands: x [n*h*wd, c] float8_e4m3fn with one fp32 scale per image (groupnorm_e4m3's
+    output), w [cout, 9*c] float8_e4m3fn with one fp32 scale per output channel (pack_e4m3_weight of the conv3x3 pack);
+    out / bias / rowvec / residual `dtype`."""
+    assert x.dtype == torch.float8_e4m3fn and w.dtype == torch.float8_e4m3fn
+    assert x_scale.dtype == torch.float32 and w_scale.dtype == torch.float32
+    c, cout = x.shape[1], w.shape[0]
+    assert x.is_contiguous() and w.is_contiguous() and w.shape[1] == 9 * c and x.shape[0] == n * h * wd
+    assert x_scale.shape == (n,) and w_scale.shape == (cout,)
+    if out is None:
+        out = torch.empty((n * h * wd, cout), dtype=dtype, device=x.device)
+    assert out.dtype == dtype and out.stride(1) == 1
+    p = L.Conv3x3E4m3Params()
+    p.x, p.x_scale, p.c_in = _ptr(x), _ptr(x_scale), c
+    p.w, p.w_scale = _ptr(w), _ptr(w_scale)
+    p.out, p.ldo = _ptr(out), out.stride(0)
+    p.n, p.h, p.w_, p.cout = n, h, wd, cout
+    p.dtype = _dt(out)
+    p.ep = _epilogue(bias, rowvec, rows_per_group or h * wd, residual, scale, act)
+    M = n * h * wd
+    with _Call("conv3x3_e4m3", 1, 2.0 * M * cout * 9 * c,
+               M * c + 9 * c * cout + 4.0 * (n + cout) + 2.0 * (M * cout + (M * cout if residual is not None else 0))):
+        L.check(L.load().mimo_conv3x3_e4m3(C.byref(p), _stream()), "mimo_conv3x3_e4m3")
+    return out
+
+
 def conv_up2x(x: torch.Tensor, w4: torch.Tensor, n: int, h: int, wd: int, *, bias=None, scale=1.0, act=L.ACT_NONE,
               out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """nearest-x2 upsample + 3x3 conv of channels-last x [n*h*wd, c] -> [n*2h*2wd, cout]; w4 from pack_conv_up2x_weight."""
@@ -326,6 +354,76 @@ def groupnorm_window_apply(x0: torch.Tensor, gamma: torch.Tensor, beta: torch.Te
     with _Call("groupnorm", 2, 0.0, 2.0 * 2 * out.numel()):
         L.check(L.load().mimo_groupnorm_window_apply(C.byref(p), _stream()), "mimo_groupnorm_window_apply")
     return out
+
+
+def _gn8(mode: int, x0, samples, frames, hw, groups, *, x1=None, gamma=None, beta=None, eps=1e-5, table=None,
+         table_frames=0, work=None, out=None, scale=None):
+    """one mimo_groupnorm_e4m3 call; returns `work` (allocated here when None)"""
+    c = x0.shape[1] + (x1.shape[1] if x1 is not None else 0)
+    assert x0.is_contiguous() and (x1 is None or x1.is_contiguous()) and x0.shape[0] == samples * frames * hw
+    p = L.GroupNormE4m3Params(mode=int(mode), samples=int(samples), frames=int(frames), table_frames=int(table_frames),
+                              hw=int(hw), groups=int(groups), eps=float(eps), dtype=_dt(x0))
+    p.x0, p.c0 = _ptr(x0), x0.shape[1]
+    p.x1, p.c1 = _ptr(x1), (x1.shape[1] if x1 is not None else 0)
+    p.gamma, p.beta, p.out, p.scale = _ptr(gamma), _ptr(beta), _ptr(out), _ptr(scale)
+    need = L.load().mimo_groupnorm_e4m3_workspace_bytes(C.byref(p))
+    if need < 0:
+        L.check(int(need), "mimo_groupnorm_e4m3_workspace_bytes")
+    if work is None:
+        work = torch.empty(((need + 3) // 4,), dtype=torch.float32, device=x0.device)
+    assert work.dtype == torch.float32 and work.is_contiguous() and work.numel() * 4 >= need
+    p.work, p.work_bytes = _ptr(work), work.numel() * 4
+    p.table, p.table_bytes = _ptr(table), (table.numel() * table.element_size() if table is not None else 0)
+    rows = samples * frames * hw
+    kernels = {L.GN_E4M3_FRAME: 2, L.GN_E4M3_WINDOW: 3, L.GN_E4M3_WINDOW_PARTIALS: 1, L.GN_E4M3_WINDOW_APPLY: 2}[mode]
+    moved = 2.0 * rows * c + (rows * c + 4.0 * samples * frames if mode != L.GN_E4M3_WINDOW_PARTIALS else 0)
+    with _Call("groupnorm_e4m3", kernels, 0.0, moved):
+        L.check(L.load().mimo_groupnorm_e4m3(C.byref(p), _stream()), "mimo_groupnorm_e4m3")
+    return work
+
+
+def _gn8_out(x0, x1, images, hw):
+    c = x0.shape[1] + (x1.shape[1] if x1 is not None else 0)
+    return (torch.empty((images * hw, c), dtype=torch.float8_e4m3fn, device=x0.device),
+            torch.empty((images,), dtype=torch.float32, device=x0.device))
+
+
+def groupnorm_e4m3(x0: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, n: int, hw: int, *, groups=32, eps=1e-5,
+                   x1: Optional[torch.Tensor] = None, window_frames: Optional[int] = None):
+    """SiLU(GroupNorm) of channels-last x0 (+ x1) quantized per image for conv3x3_e4m3: returns (q [n*hw, C]
+    float8_e4m3fn, scale [n] fp32), q * scale ~ SiLU(GroupNorm(x)) (include/mimo_b200.h and e4m3_image_scales give
+    the rule). Statistics per image, or with `window_frames` per sample over that many consecutive images."""
+    q, sc = _gn8_out(x0, x1, n, hw)
+    if window_frames is None:
+        _gn8(L.GN_E4M3_FRAME, x0, n, 1, hw, groups, x1=x1, gamma=gamma, beta=beta, eps=eps, out=q, scale=sc)
+    else:
+        f = int(window_frames)
+        c = q.shape[1]
+        table = _gnw_table(None, groupnorm_window_table_bytes(n // f, f, hw, c, groups), x0.device)
+        _gn8(L.GN_E4M3_WINDOW, x0, n // f, f, hw, groups, x1=x1, gamma=gamma, beta=beta, eps=eps, table=table,
+             table_frames=f, out=q, scale=sc)
+    return q, sc
+
+
+def groupnorm_e4m3_partials(x0: torch.Tensor, samples: int, frames: int, hw: int, *, groups=32,
+                            x1: Optional[torch.Tensor] = None, table: Optional[torch.Tensor] = None):
+    """groupnorm_window_partials() for the e4m3 output: the window table of x0's frames (same bytes as the 16-bit
+    call) and the per-frame min / max that groupnorm_e4m3_apply reads. Returns (table, work)."""
+    c = x0.shape[1] + (x1.shape[1] if x1 is not None else 0)
+    table = _gnw_table(table, groupnorm_window_table_bytes(samples, frames, hw, c, groups), x0.device)
+    work = _gn8(L.GN_E4M3_WINDOW_PARTIALS, x0, samples, frames, hw, groups, x1=x1, table=table)
+    return table, work
+
+
+def groupnorm_e4m3_apply(x0: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, table: torch.Tensor,
+                         work: torch.Tensor, samples: int, frames: int, table_frames: int, hw: int, *, groups=32,
+                         eps=1e-5, x1: Optional[torch.Tensor] = None):
+    """groupnorm_window_apply() for the e4m3 output, with the `work` of groupnorm_e4m3_partials on the same frames:
+    returns (q, scale) as groupnorm_e4m3."""
+    q, sc = _gn8_out(x0, x1, samples * frames, hw)
+    _gn8(L.GN_E4M3_WINDOW_APPLY, x0, samples, frames, hw, groups, x1=x1, gamma=gamma, beta=beta, eps=eps, table=table,
+         table_frames=table_frames, work=work, out=q, scale=sc)
+    return q, sc
 
 
 def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, *, eps=1e-5, pe: Optional[torch.Tensor] = None,
@@ -671,3 +769,50 @@ def pack_e4m3_weight(w: torch.Tensor):
     """A [N, K] weight (already in gemm's row order, e.g. pack_geglu_weight's) as (e4m3 [N, K], fp32 scale [N]): one
     scale per output channel by quantize_e4m3_rows, so the rows' order - and the GEGLU tile interleave - is kept."""
     return quantize_e4m3_rows(w)
+
+
+SILU_ARGMIN, SILU_MIN_ABS = -1.2784645, 0.27846454  # SiLU's only turning point: its minimum, silu(-1.2784645)
+
+
+def e4m3_image_scales(lo: torch.Tensor, hi: torch.Tensor, mean: torch.Tensor, rstd: torch.Tensor, gamma: torch.Tensor,
+                      beta: torch.Tensor) -> torch.Tensor:
+    """The per-image scale rule of mimo_groupnorm_e4m3 on the host. lo / hi: [n, groups] min / max of x over each image's
+    elements of a group; mean / rstd: [n, groups] the statistics the normaliser uses (the image's own, or its sample's
+    window statistics); gamma / beta: [C]. For each channel c of group g, z_lo = (lo - mean) * (rstd * gamma_c) + beta_c
+    and z_hi likewise (one rounding after the product and sum, as the kernel's fma), B_c = max(|silu(z_lo)|,
+    |silu(z_hi)|, 0.27846454 if [z_lo, z_hi] holds SiLU's minimum at -1.2784645); amax = max_c B_c and scale = amax / 448
+    (an IEEE quotient), or 1 when amax is 0. Returns (scale, inv) [n] fp32: inv = 448 / amax (1 when amax is 0) is the
+    multiplier of SiLU's output ahead of the rounding."""
+    C_ = gamma.numel()
+    g_of_c = torch.arange(C_, device=lo.device) // (C_ // lo.shape[1])
+    sc = rstd.float()[:, g_of_c] * gamma.float()[None]
+    z = [((v.float() - mean.float())[:, g_of_c].double() * sc.double() + beta.double()[None]).float() for v in (lo, hi)]
+    bnd = torch.maximum(torch.nn.functional.silu(z[0]).abs(), torch.nn.functional.silu(z[1]).abs())
+    inside = (torch.minimum(z[0], z[1]) <= SILU_ARGMIN) & (torch.maximum(z[0], z[1]) >= SILU_ARGMIN)
+    bnd = torch.where(inside, torch.clamp(bnd, min=SILU_MIN_ABS), bnd)
+    amax = bnd.amax(dim=1)
+    zero, one, top = amax == 0, torch.ones_like(amax), torch.full_like(amax, E4M3_MAX)
+    return torch.where(zero, one, amax / top), torch.where(zero, one, top / amax)
+
+
+def groupnorm_silu_e4m3_host(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, groups: int, eps: float,
+                             frames: int = 1):
+    """SiLU(GroupNorm) of x [n, hw, C] quantized per image by e4m3_image_scales, in torch (the oracle's and the tests'
+    statement of mimo_groupnorm_e4m3). Statistics per image, or with frames > 1 per sample of `frames` consecutive images
+    (fp64 sums, rounded to fp32). Returns (q [n, hw, C] float8_e4m3fn, scale [n] fp32, y = the fp32 SiLU(GroupNorm(x)))."""
+    n, hw, C_ = x.shape
+    xf = x.float()
+    xs = xf.double().reshape(n // frames, frames, hw, groups, C_ // groups)
+    mean = xs.mean(dim=(1, 2, 4))
+    var = xs.var(dim=(1, 2, 4), unbiased=False)
+    mean = mean.float().repeat_interleave(frames, 0)
+    rstd = torch.rsqrt(var.float() + eps).repeat_interleave(frames, 0)
+    xg = xf.reshape(n, hw, groups, C_ // groups)
+    lo, hi = xg.amin(dim=(1, 3)), xg.amax(dim=(1, 3))
+    scale, inv = e4m3_image_scales(lo, hi, mean, rstd, gamma, beta)
+    g_of_c = torch.arange(C_, device=x.device) // (C_ // groups)
+    sc = rstd[:, g_of_c] * gamma.float()[None]
+    y = ((xf - mean[:, g_of_c][:, None]).double() * sc[:, None].double() + beta.double()).float()
+    y = torch.nn.functional.silu(y)
+    q = torch.clamp(y * inv[:, None, None], -E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn)
+    return q, scale, y
