@@ -42,7 +42,7 @@ const char* mimo_last_error(void);
 int mimo_device_check(int dev);
 /* sizeof() of the parameter structs as compiled into the library (0 epilogue, 1 gemm, 2 conv3x3, 3 groupnorm,
  * 4 attn, 5 attn_temporal, 6 exchange, 7 cfg_multistep, 8 groupnorm_window, 9 gemm_e4m3, 10 groupnorm_e4m3,
- * 11 conv3x3_e4m3): lets a binding verify its struct mirrors before the first call. */
+ * 11 conv3x3_e4m3, 12 gemm_e4m3_geglu_e4m3, 13 gemm_e4m3_blockscaled): lets a binding verify its struct mirrors before the first call. */
 int mimo_abi_sizeof(int which);
 
 /* Fused epilogue shared by GEMM and conv:  out = act((acc + bias[c] + rowvec[row / rows_per_group][c]
@@ -114,6 +114,64 @@ typedef struct {
   int64_t workspace_bytes;
 } mimo_gemm_e4m3_params;
 int mimo_gemm_e4m3(const mimo_gemm_e4m3_params* p, void* stream);
+
+/* mimo_gemm_e4m3 with act = GEGLU whose output is e4m3 with one fp32 scale per (row, 128-column block): the A operand of
+ * mimo_gemm_e4m3_blockscaled. With v the fp32 GEGLU values of a row's block - (acc * a_scale * w_scale + bias) of the value
+ * column times gelu of the gate column's, exactly as mimo_gemm_e4m3 computes them, without a rounding to 16 bits:
+ *   amax = max |v|;  inv = 448 / amax, out_scale[block][row] = amax / 448 (IEEE divisions);  out = cvt.rn.satfinite.e4m3(v * inv)
+ * and inv = out_scale = 1 when amax == 0: the per-row rule of mimo_layernorm_e4m3, applied to each 128-column block. One
+ * GEGLU tile (256 packed weight rows) writes exactly one block of each of its rows, so the block's amax is known before
+ * any of its bytes is written. out_scale is block-major, [N / 256][ld_scale]: a tile's 128 scales are one contiguous run.
+ * Replaces, when the caller opts into the FP8 feed-forward output projection, the GEGLU of diffusers' FeedForward
+ * (src/models/attention.py:359-360, motion_module.py:235-236) ahead of mimo_gemm_e4m3_blockscaled.
+ * Requirements as mimo_gemm_e4m3 with GEGLU and a bias, and N % 256 == 0 (the 256-wide tile, weights packed with
+ * mimo_gemm_geglu_granule(N) == 128), ldo % 16 == 0 (bytes), ld_scale >= M and ld_scale % 4 == 0, no residual, no row
+ * vector, scale 1. */
+typedef struct {
+  const void* a;        /* [M, lda] e4m3 */
+  int64_t lda;
+  const float* a_scale; /* [M] */
+  const void* w;        /* [N, ldw] e4m3, GEGLU-packed */
+  int64_t ldw;
+  const float* w_scale; /* [N] */
+  const void* bias;     /* [N] `dtype`, GEGLU-packed */
+  void* out;            /* [M, ldo] e4m3, N / 2 columns */
+  int64_t ldo;
+  float* out_scale;     /* [N / 256, ld_scale] */
+  int64_t ld_scale;
+  int32_t M, N, K;
+  int32_t dtype; /* of bias */
+} mimo_gemm_e4m3_geglu_e4m3_params;
+int mimo_gemm_e4m3_geglu_e4m3(const mimo_gemm_e4m3_geglu_e4m3_params* p, void* stream);
+
+/* e4m3 GEMM with one fp32 scale per (row of A, 128-element K block) - fine-grained activation scaling - and one per
+ * output channel of W:
+ *   out[M,N] = epilogue((sum_kb a_scale[kb][m] * (A_kb . W_kb^T)[m][n]) * w_scale[n])
+ * Each K block's partial product is accumulated in fp32 on its own and added, times its row scale, into the fp32 sum
+ * (blocks in order, one fma each); w_scale is taken where the epilogue first reads the sum, then the mimo_epilogue chain
+ * runs as in mimo_gemm (bias, rowvec, residual, act NONE or SILU, scale); out, bias, rowvec and residual are `dtype`.
+ * Replaces, when the caller opts into the FP8 feed-forward output projection, FeedForward's ff.net.2 Linear(4C, C)
+ * (src/models/attention.py:359-360, motion_module.py:235-236), fed by mimo_gemm_e4m3_geglu_e4m3.
+ * Requirements: K % 128 == 0, lda / ldw % 16 == 0 (bytes), N % 8 == 0, ldo % 8 == 0, 16-byte aligned a / w / out /
+ * residual, non-NULL scales, a_scale [K / 128][ld_scale] with ld_scale >= M and ld_scale % 4 == 0, no GEGLU, no split-K
+ * (workspace must be NULL). */
+typedef struct {
+  const void* a;        /* [M, lda] e4m3 */
+  int64_t lda;
+  const float* a_scale; /* [K / 128, ld_scale] */
+  int64_t ld_scale;
+  const void* w;        /* [N, ldw] e4m3 */
+  int64_t ldw;
+  const float* w_scale; /* [N] */
+  void* out;
+  int64_t ldo;
+  int32_t M, N, K;
+  int32_t dtype; /* of out / bias / rowvec / residual */
+  mimo_epilogue ep;
+  void* workspace; /* must be NULL */
+  int64_t workspace_bytes;
+} mimo_gemm_e4m3_blockscaled_params;
+int mimo_gemm_e4m3_blockscaled(const mimo_gemm_e4m3_blockscaled_params* p, void* stream);
 
 /* 3x3 / stride 1 / pad 1 convolution as implicit GEMM: the A operand is fetched tap by tap with 4-D TMA boxes
  * over the NHWC input (out-of-bounds = zero padding), optionally from two tensors (virtual channel concat).

@@ -76,8 +76,9 @@ int encode_tmap(CUtensorMap* out, int dtype, int rank, const void* base, const u
                                                       : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   CUresult r = g_encode(out, dt, static_cast<cuuint32_t>(rank), const_cast<void*>(base), gdim, gstr, bx, es,
                         CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                                            : (swizzle_bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_128B),
+                        swizzle_bytes == 0    ? CU_TENSOR_MAP_SWIZZLE_NONE
+                        : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                              : (swizzle_bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_128B),
                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     snprintf(g_err, sizeof(g_err),
@@ -111,6 +112,8 @@ extern "C" int mimo_abi_sizeof(int which) {
     case 9: return static_cast<int>(sizeof(mimo_gemm_e4m3_params));
     case 10: return static_cast<int>(sizeof(mimo_groupnorm_e4m3_params));
     case 11: return static_cast<int>(sizeof(mimo_conv3x3_e4m3_params));
+    case 12: return static_cast<int>(sizeof(mimo_gemm_e4m3_geglu_e4m3_params));
+    case 13: return static_cast<int>(sizeof(mimo_gemm_e4m3_blockscaled_params));
   }
   return -1;
 }

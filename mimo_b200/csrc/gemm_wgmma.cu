@@ -22,6 +22,10 @@
 // same 128-byte swizzle row and stage bytes, four wgmma.m64nBNk32.e4m3 per block; the epilogue first takes
 // acc * a_scale[row] * w_scale[col] in fp32 and then runs the chain above unchanged. mimo_conv3x3_e4m3 is conv mode in
 // e4m3 (conv_e4m3_kernel): 128-channel boxes, single source, and a_scale per image of the output pixel.
+// The FP8 feed-forward adds two more e4m3 variants of the same body: mimo_gemm_e4m3_geglu_e4m3 (gemm_e4m3_geglu_e4m3_kernel)
+// ends the GEGLU epilogue in e4m3 with one scale per row and 128-column block instead of a 16-bit store, and
+// mimo_gemm_e4m3_blockscaled (gemm_blockscaled_kernel) reads A with one scale per row and 128-element K block: each K
+// block's four wgmma accumulate on their own, and the main loop adds them, times the block's row scale, into the sum.
 #include <cuda_runtime.h>
 
 #include <cudaTypedefs.h>
@@ -64,9 +68,10 @@ struct ConvGeom {
   signed char tdx[9], tdy[9];  // input offset of tap t relative to the output pixel
 };
 
-template <int BN, bool kRes, bool kE4m3 = false>
+template <int BN, bool kRes, bool kE4m3 = false, bool kBlockScale = false>
 struct GemmCfg {
-  static constexpr int kStageBytes = BM * BK * 2 + BN * BK * 2;
+  // kBlockScale: the K block's 128 fp32 row scales follow W in the stage (512 B, padded to keep stages 1024-B aligned)
+  static constexpr int kStageBytes = BM * BK * 2 + BN * BK * 2 + (kBlockScale ? 1024 : 0);
   static constexpr int kNChunk = BN / 32;
   static constexpr int kOutBytes = 2 * kChunk;  // double-buffered staging of the output chunks
   static constexpr int kResSlots = kRes ? 2 : 0;
@@ -92,6 +97,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
   constexpr bool kE4m3 = false, kImgScale = false;
   constexpr const float* a_scale = nullptr;
   constexpr const float* w_scale = nullptr;
+  constexpr bool kOutE4m3 = false, kBlockScale = false;
+  constexpr float* out_scale = nullptr;
+  constexpr long long ld_scale = 0;
+  const CUtensorMap& tmAS = tmA0;
 #include "gemm_wgmma_body.cuh"
 }
 
@@ -105,6 +114,10 @@ gemm_e4m3_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
                  int num_k_blocks, ConvGeom g, EpiArgs ep, const float* __restrict__ a_scale,
                  const float* __restrict__ w_scale) {
   constexpr bool kE4m3 = true, kImgScale = false;
+  constexpr bool kOutE4m3 = false, kBlockScale = false;
+  constexpr float* out_scale = nullptr;
+  constexpr long long ld_scale = 0;
+  const CUtensorMap& tmAS = tmA0;
 #include "gemm_wgmma_body.cuh"
 }
 
@@ -118,6 +131,42 @@ conv_e4m3_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
                  int num_k_blocks, ConvGeom g, EpiArgs ep, const float* __restrict__ a_scale,
                  const float* __restrict__ w_scale) {
   constexpr bool kE4m3 = true, kImgScale = true;
+  constexpr bool kOutE4m3 = false, kBlockScale = false;
+  constexpr float* out_scale = nullptr;
+  constexpr long long ld_scale = 0;
+  const CUtensorMap& tmAS = tmA0;
+#include "gemm_wgmma_body.cuh"
+}
+
+// GEGLU with an e4m3 output (gemm_e4m3_kernel's GEGLU, BN = 256): out_scale[n_tile][row] (row stride ld_scale) is the
+// scale of the row's 128 output columns of tile n_tile; tmOut is a one-byte map with 128 x 128 boxes
+template <bool kBf16>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_e4m3_geglu_e4m3_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
+                            const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOut,
+                            const __grid_constant__ CUtensorMap tmRes, int M, int N, int num_m_tiles, int num_n_tiles,
+                            int num_k_blocks, ConvGeom g, EpiArgs ep, const float* __restrict__ a_scale,
+                            const float* __restrict__ w_scale, float* __restrict__ out_scale, long long ld_scale) {
+  constexpr int BN = 256;
+  constexpr bool kRes = false;
+  constexpr bool kE4m3 = true, kImgScale = false, kOutE4m3 = true, kBlockScale = false;
+  const CUtensorMap& tmAS = tmA0;
+#include "gemm_wgmma_body.cuh"
+}
+
+// e4m3 A with one scale per row and 128-element K block (a_scale[kb][row], read through tmAS into the stages), W with one
+// per output channel: GEMM rows only (g.conv == 0, tmA1 == tmA0 and never read, no split-K, no GEGLU)
+template <int BN, bool kBf16, bool kRes>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_blockscaled_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
+                        const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOut,
+                        const __grid_constant__ CUtensorMap tmRes, const __grid_constant__ CUtensorMap tmAS, int M,
+                        int N, int num_m_tiles, int num_n_tiles, int num_k_blocks, ConvGeom g, EpiArgs ep,
+                        const float* __restrict__ w_scale) {
+  constexpr bool kE4m3 = true, kImgScale = false, kOutE4m3 = false, kBlockScale = true;
+  constexpr const float* a_scale = nullptr;
+  constexpr float* out_scale = nullptr;
+  constexpr long long ld_scale = 0;
 #include "gemm_wgmma_body.cuh"
 }
 
@@ -255,6 +304,10 @@ int pick_bn(int N, bool geglu, long long m_tiles);
 //   conv_e4m3_kernel<160, *, no residual / residual>: 128 / 144-148 registers, no spills
 //   conv_e4m3_kernel<256, *, *>: as gemm_e4m3_kernel<256, *, *> (the engine uses it for 1280 channels at 8 x 8)
 //   (gemm_wgmma_kernel<256, *, *>, for comparison: 168 registers, 8 B spill stores, 8-16 B spill loads)
+//   gemm_e4m3_geglu_e4m3_kernel<f16 / bf16> (BN 256, e4m3 output): 168 registers, no spills (the 96 B stack frame the
+//     spill-free kernels here all have)
+//   gemm_blockscaled_kernel<64, *, *>: 91 registers, no spills; <128, *, *>: 146 registers, no spills (two BN / 2
+//     accumulators per thread: the running sum and the K block's own)
 // e4m3 tile widths (gemm_e4m3_kernel instantiations): 192 and 256 are the widths pick_bn gives the LN-fed GEMMs of the
 // UNet (q|k|v N = 3 C: 960 / 1920 -> 192, 3840 -> 256; GEGLU N = 8 C -> 256).
 template <bool kBf16>
@@ -758,4 +811,183 @@ extern "C" int mimo_conv3x3_e4m3(const mimo_conv3x3_e4m3_params* p, void* stream
   return p->dtype == MIMO_BF16
              ? launch_conv_e4m3<true>(bn, res, m, M, p->cout, mt, nt, nkb, g, ep, p->x_scale, p->w_scale, st)
              : launch_conv_e4m3<false>(bn, res, m, M, p->cout, mt, nt, nkb, g, ep, p->x_scale, p->w_scale, st);
+}
+
+// ------------------------------------------------------------------------------------------------
+// FP8 feed-forward: GEGLU -> e4m3 blocks, block-scaled e4m3 GEMM
+// ------------------------------------------------------------------------------------------------
+// (argument checks first, then the device probe, as the other entry points)
+extern "C" int mimo_gemm_e4m3_geglu_e4m3(const mimo_gemm_e4m3_geglu_e4m3_params* p, void* stream) {
+  if (!p || !p->a || !p->w || !p->out || !p->a_scale || !p->w_scale || !p->out_scale)
+    return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_geglu_e4m3: null pointer");
+  if (p->M <= 0 || p->N <= 0 || p->K <= 0) return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_geglu_e4m3: empty problem");
+  if ((p->K % 16) || (p->lda % 16) || (p->ldw % 16) || (p->ldo % 16))
+    return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_geglu_e4m3: K, lda, ldw, ldo must be multiples of 16");
+  if (p->N % 256) return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_geglu_e4m3: N % 256 != 0 (one 128-column block per tile)");
+  if (p->ld_scale < p->M || (p->ld_scale % 4))
+    return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_geglu_e4m3: ld_scale must be >= M and a multiple of 4");
+  if ((reinterpret_cast<uintptr_t>(p->a) | reinterpret_cast<uintptr_t>(p->w) | reinterpret_cast<uintptr_t>(p->out)) % 16)
+    return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_geglu_e4m3: a, w, out must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(p->out_scale) % 16)
+    return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_geglu_e4m3: out_scale must be 16-byte aligned");
+  if (pick_bn(p->N, true, 1 << 20) != 256)
+    return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_geglu_e4m3: needs the 256-wide GEGLU tile");
+  if (int rc = ensure_device()) return rc;
+  constexpr int bn = 256;
+  const int mt = (p->M + BM - 1) / BM;
+  const int nt = p->N / bn;
+  const int nkb = (p->K + 2 * BK - 1) / (2 * BK);
+
+  Maps m;
+  const uint64_t adim[2] = {static_cast<uint64_t>(p->K), static_cast<uint64_t>(p->M)};
+  const uint64_t astr[1] = {static_cast<uint64_t>(p->lda)};
+  const uint32_t abox[2] = {2 * BK, BM};
+  if (int rc = encode_tmap(&m.a0, kTmapU8, 2, p->a, adim, astr, abox)) return rc;
+  m.a1 = m.a0;
+  const uint64_t bdim[2] = {static_cast<uint64_t>(p->K), static_cast<uint64_t>(p->N)};
+  const uint64_t bstr[1] = {static_cast<uint64_t>(p->ldw)};
+  const uint32_t bbox[2] = {2 * BK, static_cast<uint32_t>(bn)};
+  if (int rc = encode_tmap(&m.b, kTmapU8, 2, p->w, bdim, bstr, bbox)) return rc;
+  // output: one-byte elements, 128-row x 128-column boxes (one 128-byte swizzle row per tile row)
+  const uint64_t odim[2] = {static_cast<uint64_t>(p->N / 2), static_cast<uint64_t>(p->M)};
+  const uint64_t ostr[1] = {static_cast<uint64_t>(p->ldo)};
+  const uint32_t obox[2] = {2 * BK, BM};
+  if (int rc = encode_tmap(&m.out, kTmapU8, 2, p->out, odim, ostr, obox)) return rc;
+  m.res = m.out;
+  ConvGeom g = {};
+  g.kb0 = nkb;
+  g.c0 = p->K;
+  g.chunk_bytes = kChunk;
+  g.splits = 1;
+  g.kb_split = nkb;
+  mimo_epilogue e = {};
+  e.bias = p->bias;
+  e.scale = 1.0f;
+  e.act = MIMO_ACT_GEGLU;
+  const EpiArgs ep = make_epi(e, p->N);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  auto run = [&](auto kern, bool& done) -> int {
+    constexpr int smem = GemmCfg<256, false, true>::kSmemBytes;
+    if (!done) {
+      cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+      if (err != cudaSuccess) return set_cuda_error("cudaFuncSetAttribute(gemm_e4m3_geglu_e4m3)", err);
+      done = true;
+    }
+    const int tiles = mt * nt;
+    const int grid = tiles < num_sms() ? tiles : num_sms();
+    cudaError_t err = launch_k(kern, dim3(grid), dim3(kGemmThreads), smem, st, m.a0, m.a1, m.b, m.out, m.res, p->M, p->N,
+                               mt, nt, nkb, g, ep, p->a_scale, p->w_scale, p->out_scale,
+                               static_cast<long long>(p->ld_scale));
+    if (err == cudaSuccess) err = cudaGetLastError();
+    if (err != cudaSuccess) return set_cuda_error("gemm_e4m3_geglu_e4m3 launch", err);
+    return MIMO_OK;
+  };
+  static bool done[2] = {};
+  return p->dtype == MIMO_BF16 ? run(gemm_e4m3_geglu_e4m3_kernel<true>, done[1])
+                               : run(gemm_e4m3_geglu_e4m3_kernel<false>, done[0]);
+}
+
+// block-scaled tile widths (gemm_blockscaled_kernel instantiations): the per-block accumulator doubles the accumulator
+// registers, so 64 and 128 (ptxas report above). Measured on an H100 SXM (700 W) at the FF-out shapes of the 512 x 512
+// CFG window (scripts/fp8_ff_bench.py), 128 was faster at every width, even at N = 320 where it pads to 384 columns
+// (290 against 302 us at 64 x 64: 3 column tiles read each A tile 3 times instead of 5): 128, and 64 only for N <= 64.
+static int pick_bn_blockscaled(int N) {
+  if (g_force_bn) return g_force_bn;
+  return N <= 64 ? 64 : 128;
+}
+
+template <int BN, bool kBf16, bool kRes>
+static int launch_blockscaled_cfg(const Maps& m, const CUtensorMap& tas, int M, int N, int mt, int nt, int nkb,
+                                  const ConvGeom& g, const EpiArgs& ep, const float* w_scale, cudaStream_t st) {
+  constexpr int kSmem = GemmCfg<BN, kRes, true, true>::kSmemBytes;
+  auto kern = gemm_blockscaled_kernel<BN, kBf16, kRes>;
+  static bool attr_done = false;  // per instantiation
+  if (!attr_done) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
+    if (e != cudaSuccess) return set_cuda_error("cudaFuncSetAttribute(gemm_blockscaled)", e);
+    attr_done = true;
+  }
+  const int tiles = mt * nt;
+  const int grid = tiles < num_sms() ? tiles : num_sms();
+  cudaError_t e = launch_k(kern, dim3(grid), dim3(kGemmThreads), kSmem, st, m.a0, m.a1, m.b, m.out, m.res, tas, M, N, mt,
+                           nt, nkb, g, ep, w_scale);
+  if (e == cudaSuccess) e = cudaGetLastError();
+  if (e != cudaSuccess) return set_cuda_error("gemm_blockscaled launch", e);
+  return MIMO_OK;
+}
+
+template <bool kBf16>
+static int launch_blockscaled(int bn, bool res, const Maps& m, const CUtensorMap& tas, int M, int N, int mt, int nt,
+                              int nkb, const ConvGeom& g, const EpiArgs& ep, const float* w_scale, cudaStream_t st) {
+  if (bn == 64)
+    return res ? launch_blockscaled_cfg<64, kBf16, true>(m, tas, M, N, mt, nt, nkb, g, ep, w_scale, st)
+               : launch_blockscaled_cfg<64, kBf16, false>(m, tas, M, N, mt, nt, nkb, g, ep, w_scale, st);
+  return res ? launch_blockscaled_cfg<128, kBf16, true>(m, tas, M, N, mt, nt, nkb, g, ep, w_scale, st)
+             : launch_blockscaled_cfg<128, kBf16, false>(m, tas, M, N, mt, nt, nkb, g, ep, w_scale, st);
+}
+
+extern "C" int mimo_gemm_e4m3_blockscaled(const mimo_gemm_e4m3_blockscaled_params* p, void* stream) {
+  if (!p || !p->a || !p->w || !p->out || !p->a_scale || !p->w_scale)
+    return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_blockscaled: null pointer");
+  if (p->M <= 0 || p->N <= 0 || p->K <= 0) return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_blockscaled: empty problem");
+  if (p->K % 128) return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_blockscaled: K must be a multiple of 128 (the scale block)");
+  if ((p->lda % 16) || (p->ldw % 16))
+    return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_blockscaled: lda, ldw must be multiples of 16");
+  if ((p->N % 8) || (p->ldo % 8)) return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_blockscaled: N, ldo must be multiples of 8");
+  if (p->ld_scale < p->M || (p->ld_scale % 4))
+    return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_blockscaled: ld_scale must be >= M and a multiple of 4");
+  if ((reinterpret_cast<uintptr_t>(p->a) | reinterpret_cast<uintptr_t>(p->w) | reinterpret_cast<uintptr_t>(p->out) |
+       reinterpret_cast<uintptr_t>(p->a_scale) | reinterpret_cast<uintptr_t>(p->ep.residual)) % 16)
+    return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_blockscaled: a, a_scale, w, out, residual must be 16-byte aligned");
+  if (p->ep.residual && (p->ep.ld_res % 8)) return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_blockscaled: ld_res % 8 != 0");
+  if (p->ep.act == MIMO_ACT_GEGLU) return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_blockscaled: GEGLU not supported");
+  if (p->workspace || p->workspace_bytes)
+    return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_blockscaled: split-K is not supported");
+  if (g_force_bn && g_force_bn != 64 && g_force_bn != 128)
+    return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_blockscaled: unsupported BN (64 or 128)");
+  if (int rc = ensure_device()) return rc;
+  const int bn = pick_bn_blockscaled(p->N);
+  const int mt = (p->M + BM - 1) / BM;
+  const int nt = (p->N + bn - 1) / bn;
+  const int nkb = p->K / (2 * BK);
+  const bool res = p->ep.residual != nullptr;
+
+  Maps m;
+  const uint64_t adim[2] = {static_cast<uint64_t>(p->K), static_cast<uint64_t>(p->M)};
+  const uint64_t astr[1] = {static_cast<uint64_t>(p->lda)};
+  const uint32_t abox[2] = {2 * BK, BM};
+  if (int rc = encode_tmap(&m.a0, kTmapU8, 2, p->a, adim, astr, abox)) return rc;
+  m.a1 = m.a0;
+  const uint64_t bdim[2] = {static_cast<uint64_t>(p->K), static_cast<uint64_t>(p->N)};
+  const uint64_t bstr[1] = {static_cast<uint64_t>(p->ldw)};
+  const uint32_t bbox[2] = {2 * BK, static_cast<uint32_t>(bn)};
+  if (int rc = encode_tmap(&m.b, kTmapU8, 2, p->w, bdim, bstr, bbox)) return rc;
+  const uint64_t odim[2] = {static_cast<uint64_t>(p->N), static_cast<uint64_t>(p->M)};
+  const uint64_t ostr[1] = {static_cast<uint64_t>(p->ldo) * 2};
+  const uint32_t obox[2] = {32, BM};
+  if (int rc = encode_tmap(&m.out, p->dtype, 2, p->out, odim, ostr, obox, 64)) return rc;
+  m.res = m.out;
+  if (res) {
+    const uint64_t rstr[1] = {static_cast<uint64_t>(p->ep.ld_res) * 2};
+    if (int rc = encode_tmap(&m.res, p->dtype, 2, p->ep.residual, odim, rstr, obox, 64)) return rc;
+  }
+  // row scales: fp32 [K / 128][ld_scale] read as 16-bit pairs, one 128-row (512-byte) box per K block; rows past M
+  // are zero-filled
+  CUtensorMap tas;
+  {
+    const uint64_t dim[2] = {2ull * p->M, static_cast<uint64_t>(nkb)};
+    const uint64_t str[1] = {static_cast<uint64_t>(p->ld_scale) * 4};
+    const uint32_t box[2] = {2 * BM, 1};
+    if (int rc = encode_tmap(&tas, MIMO_F16, 2, p->a_scale, dim, str, box, 0)) return rc;
+  }
+  ConvGeom g = {};
+  g.kb0 = nkb;
+  g.c0 = p->K;
+  g.chunk_bytes = kChunk;
+  g.splits = 1;
+  g.kb_split = nkb;
+  const EpiArgs ep = make_epi(p->ep, p->N);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return p->dtype == MIMO_BF16 ? launch_blockscaled<true>(bn, res, m, tas, p->M, p->N, mt, nt, nkb, g, ep, p->w_scale, st)
+                               : launch_blockscaled<false>(bn, res, m, tas, p->M, p->N, mt, nt, nkb, g, ep, p->w_scale, st);
 }

@@ -1,10 +1,13 @@
 // Body of the GEMM / conv kernels of gemm_wgmma.cu (see the description at the top of that file). Not a header: the
 // kernels there include it as their whole body, so the 16-bit kernel is compiled from the same statements with the e4m3
 // steps removed by `if constexpr (kE4m3)`, and keeps its parameter list and generated code. In scope at the include:
-// the template parameters BN, kBf16, kRes, the constants kE4m3 and kImgScale, the kernel parameters tmA0, tmA1, tmB, tmOut,
-// tmRes, M, N, num_m_tiles, num_n_tiles, num_k_blocks, g, ep, and a_scale, w_scale (fp32 scales of A and W, used when
-// kE4m3: a_scale per A row, or with kImgScale per image of a convolution).
-  using Cfg = GemmCfg<BN, kRes, kE4m3>;
+// the template parameters BN, kBf16, kRes, the constants kE4m3, kImgScale, kOutE4m3 and kBlockScale, the kernel parameters
+// tmA0, tmA1, tmB, tmOut, tmRes, M, N, num_m_tiles, num_n_tiles, num_k_blocks, g, ep, and a_scale, w_scale (fp32 scales of
+// A and W, used when kE4m3: a_scale per A row, or with kImgScale per image of a convolution), out_scale and ld_scale
+// (kOutE4m3: the GEGLU output is e4m3 with one scale per row and 128-column block, out_scale[n_tile][row]), and tmAS
+// (kBlockScale: A has one scale per row and 128-element K block, a_scale[kb][row], fetched into each pipeline stage
+// through tmAS; a_scale itself is not read).
+  using Cfg = GemmCfg<BN, kRes, kE4m3, kBlockScale>;
   constexpr int kBKel = kE4m3 ? 2 * BK : BK;  // elements per K block (one 128-byte swizzle row either way)
   constexpr int kConvKel = kImgScale ? kBKel : BK;  // channels per conv K block (gemm_e4m3_kernel runs GEMM rows only)
   using C = Cvt<kBf16>;
@@ -41,6 +44,7 @@
     tma_prefetch_desc(&tmB);
     tma_prefetch_desc(&tmOut);
     if (kRes) tma_prefetch_desc(&tmRes);
+    if constexpr (kBlockScale) tma_prefetch_desc(&tmAS);
   }
   if (warp == 9 && lane == 0) {
     for (int s = 0; s < Cfg::kStages; ++s) {
@@ -89,7 +93,9 @@
         uint8_t* sb = sa + BM * BK * 2;
         if (elect_one()) {
           if (!g.conv) {
-            mbar_expect_tx(&full_bar[stage], BM * BK * 2 + BN * BK * 2);
+            mbar_expect_tx(&full_bar[stage], BM * BK * 2 + BN * BK * 2 + (kBlockScale ? BM * 4 : 0));
+            if constexpr (kBlockScale)  // the K block's 128 row scales, behind W in the stage
+              tma_load_2d(sb + BN * BK * 2, &tmAS, &full_bar[stage], 2 * m_tile * BM, kb);  // (fp32 as 16-bit pairs)
             if (kb < g.kb0) {  // A = [A0 | A1] along K (virtual concat for the up-block shortcut GEMMs)
               tma_load_2d(sa, &tmA0, &full_bar[stage], kb * kBKel, m_tile * BM);
               tma_load_2d(sb, &tmB, &full_bar[stage], kb * kBKel, n_tile * BN);
@@ -214,7 +220,9 @@
         float* sas = sbias + 1024 + (lt & 1u) * 128;
         const int col = n_tile * BN + ct;
         if (ct < BN) sws[ct] = col < N ? __ldg(w_scale + col) : 0.f;
-        if constexpr (kImgScale) {
+        if constexpr (kBlockScale) {
+          // (row scales come with each K block)
+        } else if constexpr (kImgScale) {
           // conv: one scale per image; tile row ct lies in image n0 + ct / (TW TH) of the {TW, TH, TN} footprint
           const int img = n0 + ct / (g.TW * g.TH);
           if (ct < BM) sas[ct] = img < g.NI ? __ldg(a_scale + img) : 0.f;
@@ -225,35 +233,71 @@
       }
 
       // ---- main loop: one wgmma group per k-block; the stage of k-block i - 1 is released once group i is issued ----
-      uint32_t prev_stage = 0;
-      for (int kb = 0; kb < kb_cnt; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-        const uint64_t da = make_smem_desc_sw128(sa + wg * (64 * 128), 16, 1024);
-        const uint64_t db = make_smem_desc_sw128(sa + BM * BK * 2, 16, 1024);
-        wgmma_fence();
+      // kBlockScale: each k-block's group accumulates into blk on its own; once it has completed, acc += blk * row scale
+      // of that block (the two rows of this thread), and the stage is released
+      if constexpr (kBlockScale) {
+        float blk[BN / 2];
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          // advance 32 B along K (16 16-bit / 32 e4m3 elements) inside the 128-B swizzle row: +2 in the (addr >> 4) field
-          if constexpr (kE4m3)
-            WgmmaE4m3<BN>::ss(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
-          else
-            Wgmma<BN, kBf16>::ss(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        for (int kb = 0; kb < kb_cnt; ++kb) {
+          mbar_wait(&full_bar[stage], phase);
+          uint8_t* st = smem + stage * Cfg::kStageBytes;
+          const uint32_t sa = smem_u32(st);
+          const uint64_t da = make_smem_desc_sw128(sa + wg * (64 * 128), 16, 1024);
+          const uint64_t db = make_smem_desc_sw128(sa + BM * BK * 2, 16, 1024);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < BK / 16; ++k) WgmmaE4m3<BN>::ss(blk, da + 2 * k, db + 2 * k, k != 0 ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<0>();
+          reg_fence(blk);
+          const float* srs = reinterpret_cast<const float*>(st + BM * BK * 2 + BN * BK * 2);
+          const float s0 = srs[rbase], s1 = srs[rbase + 8];
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[stage]);
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            acc[4 * j] = fmaf(blk[4 * j], s0, acc[4 * j]);
+            acc[4 * j + 1] = fmaf(blk[4 * j + 1], s0, acc[4 * j + 1]);
+            acc[4 * j + 2] = fmaf(blk[4 * j + 2], s1, acc[4 * j + 2]);
+            acc[4 * j + 3] = fmaf(blk[4 * j + 3], s1, acc[4 * j + 3]);
+          }
+          if (++stage == Cfg::kStages) {
+            stage = 0;
+            phase ^= 1u;
+          }
         }
-        wgmma_commit();
-        if (kb > 0) {
-          wgmma_wait<1>();
-          if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+      } else {
+        uint32_t prev_stage = 0;
+        for (int kb = 0; kb < kb_cnt; ++kb) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
+          const uint64_t da = make_smem_desc_sw128(sa + wg * (64 * 128), 16, 1024);
+          const uint64_t db = make_smem_desc_sw128(sa + BM * BK * 2, 16, 1024);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < BK / 16; ++k) {
+            // advance 32 B along K (16 16-bit / 32 e4m3 elements) inside the 128-B swizzle row: +2 in the (addr >> 4) field
+            if constexpr (kE4m3)
+              WgmmaE4m3<BN>::ss(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+            else
+              Wgmma<BN, kBf16>::ss(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+          }
+          wgmma_commit();
+          if (kb > 0) {
+            wgmma_wait<1>();
+            if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+          }
+          prev_stage = stage;
+          if (++stage == Cfg::kStages) {
+            stage = 0;
+            phase ^= 1u;
+          }
         }
-        prev_stage = stage;
-        if (++stage == Cfg::kStages) {
-          stage = 0;
-          phase ^= 1u;
-        }
+        wgmma_wait<0>();
+        reg_fence(acc);
+        if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
       }
-      wgmma_wait<0>();
-      reg_fence(acc);
-      if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
 
       // ---- rows of this thread; which group(s) of the per-branch vector they belong to ----
       long long row[2];
@@ -275,7 +319,7 @@
       // all BN / 2 accumulators spills at BN = 256). Split-K (ep.partial) never runs in e4m3.
       [[maybe_unused]] const float* sws = sbias + 512 + (lt & 1u) * 256;
       [[maybe_unused]] float ascale[2];
-      if constexpr (kE4m3) {
+      if constexpr (kE4m3 && !kBlockScale) {
         const float* sas = sbias + 1024 + (lt & 1u) * 128;
         ascale[0] = sas[rbase];
         ascale[1] = sas[rbase + 8];
@@ -311,7 +355,7 @@
         }
       };
 
-      if (ep.act != MIMO_ACT_GEGLU) {
+      if (!kOutE4m3 && ep.act != MIMO_ACT_GEGLU) {
         const float scale = ep.scale;
         bool rv_uniform = false;
         if (ep.rowvec) {
@@ -350,7 +394,11 @@
               const int r = rbase + 8 * h;
               const int off = r * 64 + ((jj ^ sw[h]) << 4) + q2 * 2;
               float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
-              if constexpr (kE4m3) {
+              if constexpr (kBlockScale) {  // (the row scales are in the sum already)
+                const float2 ws = *reinterpret_cast<const float2*>(sws + c * 32 + 8 * jj + q2);
+                f0 = f0 * ws.x;
+                f1 = f1 * ws.y;
+              } else if constexpr (kE4m3) {
                 const float2 ws = *reinterpret_cast<const float2*>(sws + c * 32 + 8 * jj + q2);
                 f0 = f0 * ascale[h] * ws.x;
                 f1 = f1 * ascale[h] * ws.y;
@@ -385,6 +433,56 @@
           }
           stage_and_store(obuf, col0);
         }
+      } else if constexpr (kOutE4m3) {
+        // GEGLU -> e4m3 (BN = 256): the tile's 128 output columns are one scale block. Each row's 128 values lie in the
+        // accumulators of one quad (32 per thread); they replace the value accumulators, then the row's amax is a
+        // register max and two quad shuffles, ahead of any byte. Staging: the whole 16 KiB of sOut as 128 rows of one
+        // 128-byte swizzle row each, one TMA store per tile.
+        constexpr int HALF = BN / 2;
+        static_assert(HALF == 128, "e4m3 GEGLU output: one 128-column scale block per tile");
+        float amax[2] = {0.f, 0.f};
+#pragma unroll
+        for (int j = 0; j < HALF / 8; ++j) {
+          const int jg = j + HALF / 8;
+          const float2 cv = *reinterpret_cast<const float2*>(sb + 8 * j + q2);
+          const float2 cg = *reinterpret_cast<const float2*>(sb + HALF + 8 * j + q2);
+          const float2 wv = *reinterpret_cast<const float2*>(sws + 8 * j + q2);
+          const float2 wg = *reinterpret_cast<const float2*>(sws + HALF + 8 * j + q2);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const float v0 = acc[4 * j + 2 * h] * ascale[h] * wv.x, v1 = acc[4 * j + 2 * h + 1] * ascale[h] * wv.y;
+            const float g0 = acc[4 * jg + 2 * h] * ascale[h] * wg.x, g1 = acc[4 * jg + 2 * h + 1] * ascale[h] * wg.y;
+            const float f0 = (v0 + cv.x) * gelu_erf_fast(g0 + cg.x);
+            const float f1 = (v1 + cv.y) * gelu_erf_fast(g1 + cg.y);
+            acc[4 * j + 2 * h] = f0;
+            acc[4 * j + 2 * h + 1] = f1;
+            amax[h] = fmaxf(amax[h], fmaxf(fabsf(f0), fabsf(f1)));
+          }
+        }
+        float inv[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          amax[h] = fmaxf(amax[h], __shfl_xor_sync(0xffffffffu, amax[h], 1));
+          amax[h] = fmaxf(amax[h], __shfl_xor_sync(0xffffffffu, amax[h], 2));
+          inv[h] = amax[h] == 0.f ? 1.f : 448.0f / amax[h];
+          if ((lane & 3) == 0 && row_ok[h])
+            out_scale[static_cast<long long>(n_tile) * ld_scale + row[h]] = amax[h] == 0.f ? 1.f : amax[h] / 448.0f;
+        }
+        // the previous tile's store has finished reading sOut before anyone writes it
+        if (issuer) tma_store_wait_read0();
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+#pragma unroll
+        for (int j = 0; j < HALF / 8; ++j) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = rbase + 8 * h;
+            uint16_t q;
+            asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;"
+                : "=h"(q) : "f"(acc[4 * j + 2 * h + 1] * inv[h]), "f"(acc[4 * j + 2 * h] * inv[h]));
+            *reinterpret_cast<uint16_t*>(sOut + r * 128 + (((j >> 1) ^ (r & 7)) << 4) + (j & 1) * 8 + q2) = q;
+          }
+        }
+        stage_and_store(sOut, n_tile * HALF);
       } else {
         // GEGLU: tile columns [0, BN/2) are values, [BN/2, BN) the matching gates (same thread, BN/16 fragments on)
         constexpr int HALF = BN / 2;

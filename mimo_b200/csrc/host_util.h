@@ -15,7 +15,8 @@ int ensure_device();
 int num_sms();
 // tensor-map element type for one-byte (e4m3) operands; otherwise `dtype` is MIMO_F16 / MIMO_BF16
 constexpr int kTmapU8 = 0x100;
-// rank-`rank` tiled tensor map, 16-bit (or, with kTmapU8, one-byte) elements, 128-byte swizzle, zero OOB fill.
+// rank-`rank` tiled tensor map, 16-bit (or, with kTmapU8, one-byte) elements, 128-byte swizzle (or 64, 32, 0 = none),
+// zero OOB fill.
 // dims[0] is the contiguous dimension; strides_bytes[i] is the byte stride of dims[i+1].
 int encode_tmap(CUtensorMap* out, int dtype, int rank, const void* base, const uint64_t* dims,
                 const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes = 128);

@@ -153,6 +153,9 @@ class UNetEngine:
         # set_fp8(True, convs=True): e4m3 copies of every ResnetBlock3D conv1 / conv2, in their own cache file
         self.w8c: Optional[Dict[str, dict]] = None
         self._cache8c: Optional[Path] = None
+        # set_fp8(True, ff_out=True): e4m3 copies of every feed-forward output projection (ff.net.2), in their own file
+        self.w8f: Optional[Dict[str, tuple]] = None
+        self._cache8f: Optional[Path] = None
         # packed weights: from the on-disk cache when MIMO_B200_WEIGHT_CACHE is set and holds this state dict
         from .host import weight_cache as WC
         cache = WC.cache_dir()
@@ -163,6 +166,7 @@ class UNetEngine:
             # the e4m3 copies are a function of the packed weights, which `key` already identifies: no second pass over sd
             self._cache8 = cache / f"unet-e4m3-{WC.fingerprint({}, extra=f'unet-e4m3|{key}')}.safetensors"
             self._cache8c = cache / f"unet-e4m3conv-{WC.fingerprint({}, extra=f'unet-e4m3conv|{key}')}.safetensors"
+            self._cache8f = cache / f"unet-e4m3ffo-{WC.fingerprint({}, extra=f'unet-e4m3ffo|{key}')}.safetensors"
             if cfile.exists():
                 st = WC.load(cfile, self.device)
                 self.w, self.resnets, self.xf_paths = st["w"], st["resnets"], st["xf_paths"]
@@ -293,6 +297,17 @@ class UNetEngine:
         q = ops.pack_e4m3_weight
         return {p: {"c1": q(self.w[p]["c1"][0]), "c2": q(self.w[p]["c2"][0])} for p in self.resnets}
 
+    def _pack_e4m3_ff_out(self) -> Dict[str, tuple]:
+        """e4m3 copies (one fp32 scale per output channel) of the feed-forward output projection [C, 4C] (ff.net.2) of each
+        spatial transformer and of every transformer block of each motion module, keyed as _pack_e4m3's entries"""
+        q = ops.pack_e4m3_weight
+        w8: Dict[str, tuple] = {p: q(self.w[p]["ffo"][0]) for p in self.xf_paths}
+        for p, m in self.w.items():
+            if isinstance(m, dict) and "blocks" in m:
+                for k, blk in enumerate(m["blocks"]):
+                    w8[f"{p}.{k}"] = q(blk["ffo"][0])
+        return w8
+
     def _e4m3_copies(self, cfile: Optional[Path], pack) -> Dict[str, dict]:
         from .host import weight_cache as WC
         if cfile is not None and cfile.exists():
@@ -302,25 +317,30 @@ class UNetEngine:
             WC.save(cfile, w8)
         return w8
 
-    def set_fp8(self, on: bool, convs: bool = False) -> None:
+    def set_fp8(self, on: bool, convs: bool = False, ff_out: bool = False) -> None:
         """Run the LN-fed projections (see _pack_e4m3) as LayerNorm -> e4m3 rows + scales -> e4m3 GEMM; with `convs`, also
-        every ResnetBlock3D conv1 / conv2 as GroupNorm + SiLU -> e4m3 + one scale per image -> e4m3 conv. Captured graphs
-        are dropped whenever the setting changes."""
-        on, convs = bool(on), bool(convs)
+        every ResnetBlock3D conv1 / conv2 as GroupNorm + SiLU -> e4m3 + one scale per image -> e4m3 conv; with `ff_out`,
+        also every feed-forward output projection: the e4m3 GEGLU writes e4m3 with one scale per row and 128-column
+        block, and the projection is a block-scaled e4m3 GEMM. Captured graphs are dropped whenever the setting changes."""
+        on, convs, ff_out = bool(on), bool(convs), bool(ff_out)
         if convs and not on:
             raise ValueError("set_fp8(False, convs=True): the FP8 convolutions come on top of the FP8 projections")
-        if on == self.fp8 and convs == self.fp8_convs:
+        if ff_out and not on:
+            raise ValueError("set_fp8(False, ff_out=True): the FP8 feed-forward output comes on top of the FP8 projections")
+        if on == self.fp8 and convs == self.fp8_convs and ff_out == self.fp8_ff_out:
             return
         if on and self.w8 is None:
             self.w8 = self._e4m3_copies(self._cache8, self._pack_e4m3)
         if convs and self.w8c is None:
             self.w8c = self._e4m3_copies(self._cache8c, self._pack_e4m3_convs)
-        self.fp8, self.fp8_convs = on, convs
+        if ff_out and self.w8f is None:
+            self.w8f = self._e4m3_copies(self._cache8f, self._pack_e4m3_ff_out)
+        self.fp8, self.fp8_convs, self.fp8_ff_out = on, convs, ff_out
         self._graphs.clear()
 
     def fp8_bytes(self) -> int:
-        """device bytes of the e4m3 copies (0 before the first set_fp8(True)): the projections' and, once the convs were
-        turned on, the convs'"""
+        """device bytes of the e4m3 copies (0 before the first set_fp8(True)): the projections' and, once the convs or the
+        feed-forward outputs were turned on, theirs"""
         out = 0
         for m in (self.w8 or {}).values():
             for wq, ws in [m["geglu"]] + (m["qkv"] if isinstance(m["qkv"], list) else [m["qkv"]]):
@@ -328,6 +348,8 @@ class UNetEngine:
         for m in (self.w8c or {}).values():
             for wq, ws in m.values():
                 out += wq.numel() * wq.element_size() + ws.numel() * ws.element_size()
+        for wq, ws in (self.w8f or {}).values():
+            out += wq.numel() * wq.element_size() + ws.numel() * ws.element_size()
         return out
 
     # ------------------------------------------------------------------------------------------------
@@ -388,6 +410,7 @@ class UNetEngine:
 
     _window_gn = False  # whether the forward being recorded runs the ResBlocks' GroupNorms over the window (_forward_impl)
     fp8_convs = False  # whether the ResBlock convs run from e4m3 operands (set_fp8)
+    fp8_ff_out = False  # whether the feed-forward output projections run from e4m3 operands (set_fp8)
 
     def _resnet(self, p, x0, x1, tembs, n, h, w, rows_per_branch):
         r = self.w[p]
@@ -415,12 +438,17 @@ class UNetEngine:
             res = x0
         return conv(t, "c2", residual=res)
 
-    def _ff(self, x, ln, geglu, ffo, geglu8=None):
+    def _ff(self, x, ln, geglu, ffo, geglu8=None, ffo8=None):
+        """FeedForward + residual. geglu8: LN -> e4m3 rows -> e4m3 GEGLU; ffo8 (with geglu8): the GEGLU writes e4m3 with
+        one scale per row and 128-column block, and ff.net.2 is the block-scaled e4m3 GEMM with the residual"""
         if geglu8 is None:
             nh = ops.layernorm(x, *ln)
             gg = ops.gemm(nh, geglu[0], bias=geglu[1], act=L.ACT_GEGLU)
         else:
             q, sc = ops.layernorm_e4m3(x, *ln)
+            if ffo8 is not None:
+                g8, gs = ops.gemm_e4m3_geglu_e4m3(q, sc, *geglu8, x.dtype, bias=geglu[1])
+                return ops.gemm_e4m3_blockscaled(g8, gs, *ffo8, x.dtype, bias=ffo[1], residual=x)
             gg = ops.gemm_e4m3(q, sc, *geglu8, x.dtype, bias=geglu[1], act=L.ACT_GEGLU)
         return ops.gemm(gg, ffo[0], bias=ffo[1], residual=x)
 
@@ -445,7 +473,8 @@ class UNetEngine:
             att = ops.attn_spatial(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], n, hw, self.spec.heads)
         hcur = ops.gemm(att, m["o1"][0], bias=m["o1"][1], residual=hcur, rowvec=st["xattn"][p],
                         rows_per_group=rows_per_branch)
-        hcur = self._ff(hcur, m["ln3"], m["geglu"], m["ffo"], w8["geglu"] if w8 else None)
+        hcur = self._ff(hcur, m["ln3"], m["geglu"], m["ffo"], w8["geglu"] if w8 else None,
+                        self.w8f[p] if self.fp8_ff_out else None)
         return ops.gemm(hcur, m["pout"][0], bias=m["pout"][1], residual=x)
 
     def _motion(self, p, x, b, f, hw):
@@ -486,7 +515,9 @@ class UNetEngine:
                     qkv = ops.gemm_e4m3(q, sc, *w8["qkv"][i], hcur.dtype)
                 att = ops.attn_temporal(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], b, F_, hw_l, heads)
                 hcur = ops.gemm(att, a["o"][0], bias=a["o"][1], residual=hcur)
-            hcur = self._ff(hcur, blk["ffn"], blk["geglu"], blk["ffo"], w8["geglu"] if w8 else None)
+            # (the feed-forward runs on this GPU's tokens after the exchange: no extra communication in FP8 either)
+            hcur = self._ff(hcur, blk["ffn"], blk["geglu"], blk["ffo"], w8["geglu"] if w8 else None,
+                            self.w8f[f"{p}.{k}"] if self.fp8_ff_out else None)
         if G == 1:
             return ops.gemm(hcur, m["pout"][0], bias=m["pout"][1], residual=x)
         ops.gemm(hcur, m["pout"][0], out=xg.bufs["B"].view(b * F_ * hw_l, C, x.dtype), bias=m["pout"][1])

@@ -317,24 +317,28 @@ class UNet3DConditionModel(_UNetBase):
 
     _fp8 = False
     _fp8_convs = False
+    _fp8_ff_out = False
 
-    def enable_fp8(self, convs: bool = False):
+    def enable_fp8(self, convs: bool = False, ff_out: bool = False):
         """Run the q|k|v and GEGLU projections that read a LayerNorm output in FP8 (e4m3 activations with one scale per
         token, e4m3 weights with one scale per output channel, fp32 accumulation). With `convs`, every ResnetBlock3D
         conv1 / conv2 also runs from e4m3 operands: its GroupNorm + SiLU writes e4m3 with one scale per frame, the weights
-        have one scale per output channel. Everything else stays in the model dtype. The e4m3 weight copies are made on
-        first use and kept; captured CUDA graphs of the forward are dropped."""
+        have one scale per output channel. With `ff_out`, every feed-forward output projection (ff.net.2, spatial and
+        motion) also runs from e4m3 operands: the GEGLU in front of it writes e4m3 with one scale per token and 128
+        channels, the weights have one scale per output channel. Each call sets the whole configuration. Everything else
+        stays in the model dtype. The e4m3 weight copies are made on first use and kept; captured CUDA graphs of the
+        forward are dropped."""
         if self.dtype not in (torch.float16, torch.bfloat16):
             raise MimoError(f"enable_fp8() needs an fp16 or bf16 model, not {self.dtype}")
-        self._fp8, self._fp8_convs = True, bool(convs)
+        self._fp8, self._fp8_convs, self._fp8_ff_out = True, bool(convs), bool(ff_out)
         if self._engine is not None:
-            self._engine.set_fp8(True, convs=self._fp8_convs)
+            self._engine.set_fp8(True, convs=self._fp8_convs, ff_out=self._fp8_ff_out)
         return self
 
     def disable_fp8(self):
         """Back to the model dtype for every projection and conv (the e4m3 copies stay packed for a later
         enable_fp8())."""
-        self._fp8 = self._fp8_convs = False
+        self._fp8 = self._fp8_convs = self._fp8_ff_out = False
         if self._engine is not None:
             self._engine.set_fp8(False)
         return self
@@ -347,9 +351,13 @@ class UNet3DConditionModel(_UNetBase):
     def fp8_convs_enabled(self) -> bool:
         return self._fp8_convs
 
+    @property
+    def fp8_ff_out_enabled(self) -> bool:
+        return self._fp8_ff_out
+
     def engine(self) -> E.UNetEngine:
         eng = super().engine()
-        eng.set_fp8(self._fp8, convs=self._fp8_convs)
+        eng.set_fp8(self._fp8, convs=self._fp8_convs, ff_out=self._fp8_ff_out)
         return eng
 
     @classmethod

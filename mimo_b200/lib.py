@@ -133,6 +133,33 @@ class Conv3x3E4m3Params(C.Structure):
     ]
 
 
+# FP8 feed-forward output projection (include/mimo_b200.h): GEGLU -> e4m3 with one scale per row and 128-column block,
+# which replaces the GEGLU of diffusers' FeedForward (src/models/attention.py:359-360, motion_module.py:235-236), and the
+# block-scaled e4m3 GEMM that replaces its ff.net.2 Linear(4C, C) at the same call sites
+class GemmE4m3GegluE4m3Params(C.Structure):
+    _fields_ = [
+        ("a", C.c_void_p), ("lda", C.c_int64), ("a_scale", C.c_void_p),
+        ("w", C.c_void_p), ("ldw", C.c_int64), ("w_scale", C.c_void_p),
+        ("bias", C.c_void_p),
+        ("out", C.c_void_p), ("ldo", C.c_int64),
+        ("out_scale", C.c_void_p), ("ld_scale", C.c_int64),
+        ("M", C.c_int32), ("N", C.c_int32), ("K", C.c_int32),
+        ("dtype", C.c_int32),
+    ]
+
+
+class GemmE4m3BlockscaledParams(C.Structure):
+    _fields_ = [
+        ("a", C.c_void_p), ("lda", C.c_int64), ("a_scale", C.c_void_p), ("ld_scale", C.c_int64),
+        ("w", C.c_void_p), ("ldw", C.c_int64), ("w_scale", C.c_void_p),
+        ("out", C.c_void_p), ("ldo", C.c_int64),
+        ("M", C.c_int32), ("N", C.c_int32), ("K", C.c_int32),
+        ("dtype", C.c_int32),
+        ("ep", Epilogue),
+        ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64),
+    ]
+
+
 class AttnParams(C.Structure):
     _fields_ = [
         ("q", C.c_void_p), ("k", C.c_void_p), ("v", C.c_void_p), ("ld_qkv", C.c_int64),
@@ -193,6 +220,8 @@ SYMBOLS = {
     "mimo_gemm": (C.c_int, [C.POINTER(GemmParams), _VP]),
     "mimo_gemm_geglu_granule": (C.c_int, [_I32]),
     "mimo_gemm_e4m3": (C.c_int, [C.POINTER(GemmE4m3Params), _VP]),
+    "mimo_gemm_e4m3_geglu_e4m3": (C.c_int, [C.POINTER(GemmE4m3GegluE4m3Params), _VP]),
+    "mimo_gemm_e4m3_blockscaled": (C.c_int, [C.POINTER(GemmE4m3BlockscaledParams), _VP]),
     "mimo_conv3x3": (C.c_int, [C.POINTER(Conv3x3Params), _VP]),
     "mimo_conv_up2x": (C.c_int, [C.POINTER(Conv3x3Params), _VP]),
     "mimo_conv3x3_e4m3": (C.c_int, [C.POINTER(Conv3x3E4m3Params), _VP]),
@@ -252,7 +281,8 @@ def load() -> C.CDLL:
         fn.argtypes = args
     for which, st in enumerate((Epilogue, GemmParams, Conv3x3Params, GroupNormParams, AttnParams, AttnTemporalParams,
                              ExchangeParams, CfgMultistepParams, GroupNormWindowParams, GemmE4m3Params,
-                             GroupNormE4m3Params, Conv3x3E4m3Params)):
+                             GroupNormE4m3Params, Conv3x3E4m3Params, GemmE4m3GegluE4m3Params,
+                             GemmE4m3BlockscaledParams)):
         if lib.mimo_abi_sizeof(which) != C.sizeof(st):
             raise MimoError(f"ABI mismatch: {st.__name__} is {C.sizeof(st)} bytes in lib.py but "
                             f"{lib.mimo_abi_sizeof(which)} in {LIB_PATH.name}; rebuild the library")

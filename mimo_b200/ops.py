@@ -155,6 +155,70 @@ def gemm_e4m3(a: torch.Tensor, a_scale: torch.Tensor, w: torch.Tensor, w_scale: 
     return out
 
 
+E4M3_BLOCK = 128  # K elements per activation scale of gemm_e4m3_blockscaled (one GEGLU tile's output columns)
+
+
+def gemm_e4m3_geglu_e4m3(a: torch.Tensor, a_scale: torch.Tensor, w: torch.Tensor, w_scale: torch.Tensor,
+                         dtype: torch.dtype, *, bias=None):
+    """gemm_e4m3(..., act=GEGLU) with an e4m3 output: returns (q [M, N/2] float8_e4m3fn, scale [N/2 / 128, M] fp32),
+    q[:, 128 b:128 b + 128] * scale[b][:, None] ~ the fp32 GEGLU values, quantized per row and 128-column block by
+    quantize_e4m3_blocks' rule (include/mimo_b200.h). w is the GEGLU-packed e4m3 weight (N % 256 == 0), bias `dtype`."""
+    assert a.dtype == torch.float8_e4m3fn and w.dtype == torch.float8_e4m3fn
+    assert a.dim() == 2 and w.dim() == 2 and a.shape[1] == w.shape[1] and a.stride(1) == 1 and w.stride(1) == 1
+    assert a_scale.dtype == torch.float32 and w_scale.dtype == torch.float32
+    assert a_scale.shape == (a.shape[0],) and w_scale.shape == (w.shape[0],)
+    M, K = a.shape
+    N = w.shape[0]
+    lds = (M + 3) // 4 * 4
+    out = torch.empty((M, N // 2), dtype=torch.float8_e4m3fn, device=a.device)
+    sc = torch.empty((N // 2 // E4M3_BLOCK, lds), dtype=torch.float32, device=a.device)
+    p = L.GemmE4m3GegluE4m3Params()
+    p.a, p.lda, p.a_scale = _ptr(a), a.stride(0), _ptr(a_scale)
+    p.w, p.ldw, p.w_scale = _ptr(w), w.stride(0), _ptr(w_scale)
+    p.bias = _ptr(bias) if bias is not None else None
+    if bias is not None:
+        assert bias.dtype == dtype and bias.shape == (N,)
+    p.out, p.ldo = _ptr(out), out.stride(0)
+    p.out_scale, p.ld_scale = _ptr(sc), lds
+    p.M, p.N, p.K = M, N, K
+    p.dtype = L.BF16 if dtype == torch.bfloat16 else L.F16
+    with _Call("gemm_e4m3_geglu_e4m3", 1, 2.0 * M * N * K, M * K + N * K + 4.0 * (M + N) + M * N // 2 + 4.0 * M * N / 256):
+        L.check(L.load().mimo_gemm_e4m3_geglu_e4m3(C.byref(p), _stream()), "mimo_gemm_e4m3_geglu_e4m3")
+    return out, sc[:, :M]
+
+
+def gemm_e4m3_blockscaled(a: torch.Tensor, a_scale: torch.Tensor, w: torch.Tensor, w_scale: torch.Tensor,
+                          dtype: torch.dtype, out: Optional[torch.Tensor] = None, *, bias=None, rowvec=None,
+                          rows_per_group=1, residual=None, scale=1.0, act=L.ACT_NONE) -> torch.Tensor:
+    """out[M, N] = epilogue((sum_b (a_b @ w_b^T) * a_scale[b][:, None]) * w_scale[None, :]) over the 128-wide K blocks b:
+    a [M, K] float8_e4m3fn with a_scale [K / 128, M] fp32 (gemm_e4m3_geglu_e4m3's output), w [N, K] float8_e4m3fn with one
+    fp32 scale per row (pack_e4m3_weight); out / bias / residual `dtype`."""
+    assert a.dtype == torch.float8_e4m3fn and w.dtype == torch.float8_e4m3fn
+    assert a.dim() == 2 and w.dim() == 2 and a.shape[1] == w.shape[1] and a.stride(1) == 1 and w.stride(1) == 1
+    assert a_scale.dtype == torch.float32 and w_scale.dtype == torch.float32
+    M, K = a.shape
+    N = w.shape[0]
+    assert a_scale.shape == (K // E4M3_BLOCK, M) and w_scale.shape == (N,)
+    if a_scale.stride(1) != 1 or a_scale.stride(0) % 4 or a_scale.data_ptr() % 16:  # rows of whole 16-byte groups
+        lds = (M + 3) // 4 * 4
+        a_scale = torch.zeros((K // E4M3_BLOCK, lds), dtype=torch.float32, device=a.device)[:, :M].copy_(a_scale)
+    if out is None:
+        out = torch.empty((M, N), dtype=dtype, device=a.device)
+    assert out.shape == (M, N) and out.stride(1) == 1 and out.dtype == dtype
+    p = L.GemmE4m3BlockscaledParams()
+    p.a, p.lda = _ptr(a), a.stride(0)
+    p.a_scale, p.ld_scale = _ptr(a_scale), a_scale.stride(0) if a_scale.shape[0] > 1 else (M + 3) // 4 * 4
+    p.w, p.ldw, p.w_scale = _ptr(w), w.stride(0), _ptr(w_scale)
+    p.out, p.ldo = _ptr(out), out.stride(0)
+    p.M, p.N, p.K = M, N, K
+    p.dtype = _dt(out)
+    p.ep = _epilogue(bias, rowvec, rows_per_group, residual, scale, act)
+    with _Call("gemm_e4m3_blockscaled", 1, 2.0 * M * N * K,
+               M * K + N * K + 4.0 * (M * K / E4M3_BLOCK + N) + 2.0 * (M * N + (M * N if residual is not None else 0))):
+        L.check(L.load().mimo_gemm_e4m3_blockscaled(C.byref(p), _stream()), "mimo_gemm_e4m3_blockscaled")
+    return out
+
+
 def conv3x3(x0: torch.Tensor, w: torch.Tensor, n: int, h: int, wd: int, out: Optional[torch.Tensor] = None, *,
             x1: Optional[torch.Tensor] = None, bias=None, rowvec=None, rows_per_group: Optional[int] = None,
             residual=None, scale=1.0, act=L.ACT_NONE) -> torch.Tensor:
@@ -763,6 +827,16 @@ def quantize_e4m3_rows(y: torch.Tensor):
     scale = torch.where(zero, torch.ones_like(amax), amax / torch.full_like(amax, E4M3_MAX))
     q = torch.clamp(y * inv[:, None], -E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn)
     return q.contiguous(), scale.contiguous()
+
+
+def quantize_e4m3_blocks(y: torch.Tensor, block: int = E4M3_BLOCK):
+    """The per-(row, block) e4m3 rule of mimo_gemm_e4m3_geglu_e4m3 on the host: quantize_e4m3_rows applied to each run of
+    `block` consecutive columns of each row of y [M, K] (K % block == 0), with the same tensor / tensor divisions. Returns
+    (q [M, K] float8_e4m3fn, scale [K / block, M] fp32, block-major as the kernel writes it)."""
+    M, K = y.shape
+    assert K % block == 0
+    q, s = quantize_e4m3_rows(y.float().reshape(M * (K // block), block))
+    return q.reshape(M, K).contiguous(), s.reshape(M, K // block).t().contiguous()
 
 
 def pack_e4m3_weight(w: torch.Tensor):
