@@ -42,7 +42,8 @@ const char* mimo_last_error(void);
 int mimo_device_check(int dev);
 /* sizeof() of the parameter structs as compiled into the library (0 epilogue, 1 gemm, 2 conv3x3, 3 groupnorm,
  * 4 attn, 5 attn_temporal, 6 exchange, 7 cfg_multistep, 8 groupnorm_window, 9 gemm_e4m3, 10 groupnorm_e4m3,
- * 11 conv3x3_e4m3, 12 gemm_e4m3_geglu_e4m3, 13 gemm_e4m3_blockscaled): lets a binding verify its struct mirrors before the first call. */
+ * 11 conv3x3_e4m3, 12 gemm_e4m3_geglu_e4m3, 13 gemm_e4m3_blockscaled, 14 cfg_rescale): lets a binding verify its struct
+ * mirrors before the first call. */
 int mimo_abi_sizeof(int which);
 
 /* Fused epilogue shared by GEMM and conv:  out = act((acc + bias[c] + rowvec[row / rows_per_group][c]
@@ -522,6 +523,34 @@ typedef struct {
 } mimo_cfg_multistep_params;
 /* Requirements: finite scalars; hist_out distinct from latents, pred_*, h1 and noise. Graph-capturable. */
 int mimo_cfg_multistep(const mimo_cfg_multistep_params* p, void* stream);
+
+/* Rescaled classifier-free guidance (Lin et al. 2023, arXiv 2305.08891 §3.4; diffusers rescale_noise_cfg [3P]) at the
+ * point where diffusers' pipelines apply it in the reference's loop: after the guidance line, before the scheduler step
+ * (pipeline_pose2vid_long_edit_bkfill_roiclip.py:545-553). With text = pred_cond / counter and cfg the guided prediction,
+ * both computed exactly as mimo_cfg_ddim_step computes them:
+ *   r   = rnd(rnd(std(text)) / rnd(std(cfg)))        std unbiased over all `count` elements (the whole clip); r = 1 when
+ *                                                    rnd(std(cfg)) is 0 (diffusers would give NaN)
+ *   out = rnd(rnd(phi * rnd(cfg * r)) + rnd((1 - phi) * cfg))   phi and 1 - phi in double, cast to fp32
+ * rnd rounds to `dtype`, where PyTorch rounds that expression on 16-bit tensors. The sums behind the two std are fp64, one
+ * fixed partial per CTA in `workspace`, added in a fixed order by a grid whose size depends on `count` only: repeated
+ * calls, graph replays and every rank of a sharded run give the same bits. No host synchronisation; graph-capturable.
+ * Two kernel launches. The scheduler step then runs on (out, out, guidance 1, no counter), which passes out through. */
+typedef struct {
+  const void* pred_uncond; /* [count]                                                                      */
+  const void* pred_cond;   /* [count]                                                                      */
+  const void* counter;     /* [F] window count per frame (as mimo_cfg_ddim_step), or NULL                  */
+  int64_t frame_stride;    /* h * w: latents are [1, 4, F, h, w]; needed with counter                      */
+  void* out;               /* [count] in `dtype`; distinct from every input                               */
+  int64_t count;           /* >= 2                                                                         */
+  void* workspace;         /* mimo_cfg_rescale_workspace_bytes(p) bytes, 16-byte aligned, contents irrelevant  */
+  int64_t workspace_bytes;
+  double phi;              /* guidance_rescale, in [0, 1]                                                  */
+  float guidance;          /* finite                                                                       */
+  int32_t dtype;
+} mimo_cfg_rescale_params;
+int mimo_cfg_rescale(const mimo_cfg_rescale_params* p, void* stream);
+/* bytes of `workspace` mimo_cfg_rescale needs for p->count (pointers in *p are ignored); < 0 on a bad count */
+int64_t mimo_cfg_rescale_workspace_bytes(const mimo_cfg_rescale_params* p);
 
 /* Latent frame interpolation (pipeline interpolate_latents, :294-334, with the methods of src/pipelines/utils.py):
  * src [1, 4, F, h, w] -> dst [1, 4, (F-1)*k + 1, h, w] (hw = h * w): frame i goes to i*k, and k-1 frames

@@ -114,6 +114,7 @@ extern "C" int mimo_abi_sizeof(int which) {
     case 11: return static_cast<int>(sizeof(mimo_conv3x3_e4m3_params));
     case 12: return static_cast<int>(sizeof(mimo_gemm_e4m3_geglu_e4m3_params));
     case 13: return static_cast<int>(sizeof(mimo_gemm_e4m3_blockscaled_params));
+    case 14: return static_cast<int>(sizeof(mimo_cfg_rescale_params));
   }
   return -1;
 }

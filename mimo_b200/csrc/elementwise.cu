@@ -218,6 +218,22 @@ __global__ void ew_kernel(const void* __restrict__ a, const void* __restrict__ b
   }
 }
 
+// The reference's guidance line (pipeline :545-549) on element i, rounded where its torch expression rounds in the storage
+// type: (noise_pred / counter).chunk(2) when a per-frame counter is given, then u + g * (c - u). Leaves u and c as the
+// divided halves (c is diffusers' noise_pred_text). Shared by every CFG kernel so that they guide identically.
+template <bool kBf16>
+__device__ __forceinline__ float cfg_guide(float& u, float& c, const typename Cvt<kBf16>::T* cnt, long long i,
+                                           long long frame_stride, int frames, float g) {
+  using C = Cvt<kBf16>;
+  auto rnd = [](float v) { return C::to_f(C::from_f(v)); };
+  if (cnt) {
+    const float n = C::to_f(cnt[(i / frame_stride) % frames]);
+    u = rnd(u / n);
+    c = rnd(c / n);
+  }
+  return rnd(u + rnd(g * rnd(c - u)));
+}
+
 // CFG + DDIM (v-prediction). Every intermediate is rounded to the storage type where the reference's torch expression
 // would round it (it runs the whole update in the latents' dtype). kNoise: stochastic DDIM (eta > 0): s1a_p is then the
 // direction coefficient sqrt(1 - abar_prev - sigma^2), and sigma * noise is added last, as DDIMScheduler.step [3P] does.
@@ -233,12 +249,7 @@ __global__ void cfg_ddim_kernel(const void* __restrict__ pu, const void* __restr
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     float u = C::to_f(static_cast<const T*>(pu)[i]);
     float c = C::to_f(static_cast<const T*>(pc)[i]);
-    if (counter) {
-      const float cnt = C::to_f(static_cast<const T*>(counter)[(i / frame_stride) % frames]);
-      u = rnd(u / cnt);
-      c = rnd(c / cnt);
-    }
-    const float v = rnd(u + rnd(g * rnd(c - u)));
+    const float v = cfg_guide<kBf16>(u, c, static_cast<const T*>(counter), i, frame_stride, frames, g);
     const float x = C::to_f(static_cast<T*>(lat)[i]);
     // DDIMScheduler.step: alpha terms are fp32 scalars -> products promote to fp32 only for 0-dim tensors'
     // python floats; tensor math stays in the storage dtype
@@ -258,7 +269,6 @@ template <bool kBf16>
 __global__ void cfg_multistep_kernel(const mimo_cfg_multistep_params p, int frames) {
   using C = Cvt<kBf16>;
   using T = typename C::T;
-  auto rnd = [](float v) { return C::to_f(C::from_f(v)); };
   const T* __restrict__ pu = static_cast<const T*>(p.pred_uncond);
   const T* __restrict__ pc = static_cast<const T*>(p.pred_cond);
   const T* __restrict__ cnt = static_cast<const T*>(p.counter);
@@ -271,12 +281,7 @@ __global__ void cfg_multistep_kernel(const mimo_cfg_multistep_params p, int fram
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     float u = C::to_f(pu[i]);
     float c = C::to_f(pc[i]);
-    if (cnt) {
-      const float n = C::to_f(cnt[(i / p.frame_stride) % frames]);
-      u = rnd(u / n);
-      c = rnd(c / n);
-    }
-    const float v = rnd(u + rnd(p.guidance * rnd(c - u)));
+    const float v = cfg_guide<kBf16>(u, c, cnt, i, p.frame_stride, frames, p.guidance);
     const float x = C::to_f(lat[i]);
     const T mt = C::from_f(fmaf(p.a, x, p.b * v));
     const float m = C::to_f(mt);
@@ -286,6 +291,100 @@ __global__ void cfg_multistep_kernel(const mimo_cfg_multistep_params p, int fram
     if (nz) acc = fmaf(p.c_n, C::to_f(nz[i]), acc);
     hist[i] = mt;
     lat[i] = C::from_f(acc);
+  }
+}
+
+// Rescaled CFG (mimo_cfg_rescale), two launches of the same count-only grid. The statistics pass writes one fixed
+// partial per CTA (sum and sum of squares of the text half and of the guided value, fp64); the apply pass has every CTA
+// add all partials in the same fixed order, so each derives bit-identical statistics with no atomics and no host sync.
+constexpr int kRescaleThreads = 256;
+constexpr long long kRescaleElemsPerCta = 4096;
+constexpr int kRescaleMaxCtas = 256;  // the apply pass re-reads at most 256 x 32 B of partials per CTA
+
+static inline int cfg_rescale_ctas(long long count) {
+  const long long b = (count + kRescaleElemsPerCta - 1) / kRescaleElemsPerCta;
+  return static_cast<int>(b < 1 ? 1 : (b > kRescaleMaxCtas ? kRescaleMaxCtas : b));
+}
+
+// sums s[0..3] over the CTA: fixed xor-shuffle tree per warp, then every thread adds the warp totals in warp order
+__device__ __forceinline__ void cta_sum4(double (&s)[4], double (*red)[kRescaleThreads / 32]) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    for (int o = 16; o > 0; o >>= 1) s[k] += __shfl_xor_sync(0xffffffffu, s[k], o);
+  if ((threadIdx.x & 31) == 0)
+#pragma unroll
+    for (int k = 0; k < 4; ++k) red[k][threadIdx.x >> 5] = s[k];
+  __syncthreads();
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    s[k] = 0.0;
+    for (int w = 0; w < kRescaleThreads / 32; ++w) s[k] += red[k][w];
+  }
+}
+
+template <bool kBf16>
+__global__ void __launch_bounds__(kRescaleThreads) cfg_rescale_stats_kernel(const mimo_cfg_rescale_params p,
+                                                                              int frames) {
+  using C = Cvt<kBf16>;
+  using T = typename C::T;
+  __shared__ double red[4][kRescaleThreads / 32];
+  const T* __restrict__ pu = static_cast<const T*>(p.pred_uncond);
+  const T* __restrict__ pc = static_cast<const T*>(p.pred_cond);
+  const T* __restrict__ cnt = static_cast<const T*>(p.counter);
+  double s[4] = {0.0, 0.0, 0.0, 0.0};
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < p.count;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    float u = C::to_f(pu[i]);
+    float c = C::to_f(pc[i]);
+    const double g = cfg_guide<kBf16>(u, c, cnt, i, p.frame_stride, frames, p.guidance);
+    const double t = c;
+    s[0] += t;
+    s[1] = fma(t, t, s[1]);
+    s[2] += g;
+    s[3] = fma(g, g, s[3]);
+  }
+  cta_sum4(s, red);
+  if (threadIdx.x == 0) {
+    double* part = static_cast<double*>(p.workspace) + 4LL * blockIdx.x;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) part[k] = s[k];
+  }
+}
+
+// out = phi * rnd(cfg * r) + (1 - phi) * cfg, r = rnd(rnd(std(text)) / rnd(std(cfg))) (r = 1 when std(cfg) rounds to 0),
+// each product and the sum rounded to the storage type: diffusers' rescale_noise_cfg [3P] evaluated by PyTorch in that
+// type. w1 / w0 are phi and 1 - phi, computed in double and cast to fp32 as PyTorch casts a Python scalar.
+template <bool kBf16>
+__global__ void __launch_bounds__(kRescaleThreads) cfg_rescale_apply_kernel(const mimo_cfg_rescale_params p,
+                                                                              int frames, int parts, float w1,
+                                                                              float w0) {
+  using C = Cvt<kBf16>;
+  using T = typename C::T;
+  auto rnd = [](float v) { return C::to_f(C::from_f(v)); };
+  __shared__ double red[4][kRescaleThreads / 32];
+  const T* __restrict__ pu = static_cast<const T*>(p.pred_uncond);
+  const T* __restrict__ pc = static_cast<const T*>(p.pred_cond);
+  const T* __restrict__ cnt = static_cast<const T*>(p.counter);
+  T* __restrict__ out = static_cast<T*>(p.out);
+  const double* __restrict__ part = static_cast<const double*>(p.workspace);
+  double s[4] = {0.0, 0.0, 0.0, 0.0};
+  for (int j = threadIdx.x; j < parts; j += blockDim.x)
+#pragma unroll
+    for (int k = 0; k < 4; ++k) s[k] += part[4LL * j + k];
+  cta_sum4(s, red);
+  // unbiased variance (torch.std's default); a constant input may cancel to a tiny negative value
+  const double n = static_cast<double>(p.count);
+  const double var_t = fmax((s[1] - s[0] * s[0] / n) / (n - 1.0), 0.0);
+  const double var_g = fmax((s[3] - s[2] * s[2] / n) / (n - 1.0), 0.0);
+  const float std_t = rnd(static_cast<float>(sqrt(var_t)));
+  const float std_g = rnd(static_cast<float>(sqrt(var_g)));
+  const float r = std_g == 0.f ? 1.f : rnd(__fdiv_rn(std_t, std_g));
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < p.count;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    float u = C::to_f(pu[i]);
+    float c = C::to_f(pc[i]);
+    const float g = cfg_guide<kBf16>(u, c, cnt, i, p.frame_stride, frames, p.guidance);
+    out[i] = C::from_f(__fadd_rn(rnd(__fmul_rn(w1, rnd(__fmul_rn(g, r)))), rnd(__fmul_rn(w0, g))));
   }
 }
 
@@ -627,6 +726,47 @@ extern "C" int mimo_cfg_multistep(const mimo_cfg_multistep_params* p, void* stre
   else
     cfg_multistep_kernel<false><<<ew_grid(p->count, 256), 256, 0, st>>>(*p, frames);
   MIMO_CHECK_LAUNCH("cfg_multistep launch");
+  return MIMO_OK;
+}
+
+extern "C" int64_t mimo_cfg_rescale_workspace_bytes(const mimo_cfg_rescale_params* p) {
+  if (!p) return set_error(MIMO_ERR_ARG, "mimo_cfg_rescale_workspace_bytes: null params");
+  if (p->count < 2) return set_error(MIMO_ERR_ARG, "mimo_cfg_rescale_workspace_bytes: count < 2");
+  return 4LL * static_cast<long long>(sizeof(double)) * cfg_rescale_ctas(p->count);
+}
+
+extern "C" int mimo_cfg_rescale(const mimo_cfg_rescale_params* p, void* stream) {
+  if (!p || !p->pred_uncond || !p->pred_cond || !p->out || !p->workspace)
+    return set_error(MIMO_ERR_ARG, "mimo_cfg_rescale: null pointer");
+  if (p->count < 2) return set_error(MIMO_ERR_ARG, "mimo_cfg_rescale: count < 2 (the standard deviation is unbiased)");
+  if (p->dtype != MIMO_F16 && p->dtype != MIMO_BF16) return set_error(MIMO_ERR_ARG, "mimo_cfg_rescale: bad dtype");
+  if (!std::isfinite(p->guidance)) return set_error(MIMO_ERR_ARG, "mimo_cfg_rescale: non-finite guidance");
+  if (!(p->phi >= 0.0 && p->phi <= 1.0)) return set_error(MIMO_ERR_ARG, "mimo_cfg_rescale: phi must be in [0, 1]");
+  int frames = 1;
+  if (p->counter) {
+    if (p->frame_stride <= 0 || p->count % (4 * p->frame_stride))
+      return set_error(MIMO_ERR_ARG, "mimo_cfg_rescale: bad frame_stride");
+    frames = static_cast<int>(p->count / (4 * p->frame_stride));
+  }
+  const int parts = cfg_rescale_ctas(p->count);
+  if (p->workspace_bytes < 4LL * static_cast<long long>(sizeof(double)) * parts ||
+      (reinterpret_cast<uintptr_t>(p->workspace) & 15))
+    return set_error(MIMO_ERR_ARG, "mimo_cfg_rescale: workspace smaller than mimo_cfg_rescale_workspace_bytes or "
+                                   "not 16-byte aligned");
+  const void* o = p->out;
+  if (o == p->pred_uncond || o == p->pred_cond || o == p->counter || o == p->workspace)
+    return set_error(MIMO_ERR_ARG, "mimo_cfg_rescale: out aliases pred_uncond, pred_cond, counter or workspace");
+  if (int rc = ensure_device()) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const float w1 = static_cast<float>(p->phi), w0 = static_cast<float>(1.0 - p->phi);
+  if (p->dtype == MIMO_BF16) {
+    cfg_rescale_stats_kernel<true><<<parts, kRescaleThreads, 0, st>>>(*p, frames);
+    cfg_rescale_apply_kernel<true><<<parts, kRescaleThreads, 0, st>>>(*p, frames, parts, w1, w0);
+  } else {
+    cfg_rescale_stats_kernel<false><<<parts, kRescaleThreads, 0, st>>>(*p, frames);
+    cfg_rescale_apply_kernel<false><<<parts, kRescaleThreads, 0, st>>>(*p, frames, parts, w1, w0);
+  }
+  MIMO_CHECK_LAUNCH("cfg_rescale launch");
   return MIMO_OK;
 }
 

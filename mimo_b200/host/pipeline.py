@@ -436,14 +436,17 @@ class Pose2VideoPipeline:
     def sample_tensors(self, inp: Dict[str, torch.Tensor], num_inference_steps: int, guidance_scale: float,
                        context_schedule="uniform", context_frames=24, context_stride=1, context_overlap=4,
                        callback=None, callback_steps=1, decode: bool = True, eta: float = 0.0,
-                       interpolation_factor: int = 1) -> Dict[str, torch.Tensor]:
+                       interpolation_factor: int = 1, guidance_rescale: float = 0.0) -> Dict[str, torch.Tensor]:
         """Device side: everything in `inp` already lives in HBM; returns device tensors. The scheduler is
         engine_scheduler(self.scheduler); each step is one fused kernel: mimo_cfg_ddim_step(_noise) for DDIM,
         mimo_cfg_multistep for DPM-Solver++, Euler and Euler-ancestral. The per-step noise of eta > 0 (stochastic DDIM)
         and of Euler-ancestral is inp["step_noise"] [steps, 1, 4, F, h, w] (preprocess draws it from the generator) or,
         without it, drawn on the device at every step. interpolation_factor k >= 2: the registered interpolation method
-        inserts k-1 frames between neighbours before the decode; out["latents"] stays the denoised clip."""
-        sched, interp, step_noise = self._check_sampling(inp, num_inference_steps, eta, interpolation_factor)
+        inserts k-1 frames between neighbours before the decode; out["latents"] stays the denoised clip.
+        guidance_rescale phi in [0, 1]: rescaled CFG (Lin et al. 2023 §3.4, diffusers' rescale_noise_cfg [3P]) between
+        the guidance line and the step, with statistics over the whole clip (mimo_cfg_rescale); 0 or no CFG: not run."""
+        sched, interp, step_noise = self._check_sampling(inp, num_inference_steps, eta, interpolation_factor,
+                                                         guidance_rescale)
         dtype, do_cfg = self.denoising_unet.dtype, guidance_scale > 1.0
         marks = []
 
@@ -470,7 +473,7 @@ class Pose2VideoPipeline:
         reader, writer = self._reference_pass(ref_latents, ehs, do_cfg, branches, dtype)
         mark("reference_unet")
         self._denoise(sched, timesteps, latents, windows, plan, branches, pose_fea, vid_bk, guidance_scale, eta,
-                      step_noise, callback, callback_steps)
+                      step_noise, callback, callback_steps, guidance_rescale)
         mark("denoise")
         reader.clear()
         writer.clear()
@@ -486,10 +489,18 @@ class Pose2VideoPipeline:
         self.last_latents = latents
         return out
 
-    def _check_sampling(self, inp, num_inference_steps: int, eta: float, interpolation_factor: int):
+    @staticmethod
+    def _check_guidance_rescale(guidance_rescale: float) -> None:
+        """phi of rescaled CFG must lie in the paper's range [0, 1] (NaN and infinities refused)."""
+        if not 0.0 <= float(guidance_rescale) <= 1.0:
+            raise ValueError(f"guidance_rescale={guidance_rescale}: must be a finite value in [0, 1]")
+
+    def _check_sampling(self, inp, num_inference_steps: int, eta: float, interpolation_factor: int,
+                        guidance_rescale: float = 0.0):
         """The refusals, in this order, before any work -> (scheduler, interpolation method, step noise or None)."""
         if eta < 0:
             raise ValueError(f"eta={eta}: DDIM's eta is >= 0 (0 deterministic, 1 DDPM-like)")
+        self._check_guidance_rescale(guidance_rescale)
         interp = self._interpolation_method(interpolation_factor, inp["latents"].shape[2])
         sched = engine_scheduler(self.scheduler)
         step_noise = inp.get("step_noise") if sched.step_draws(eta) else None
@@ -565,11 +576,14 @@ class Pose2VideoPipeline:
         return reader, writer
 
     def _denoise(self, sched, timesteps, latents, windows, plan, branches, pose_fea, vid_bk, guidance_scale: float,
-                 eta: float, step_noise, callback, callback_steps: int) -> None:
-        """The denoising loop (pipeline :492-561) on `latents`, in place: per step, this GPU's windows, then fused_step."""
+                 eta: float, step_noise, callback, callback_steps: int, guidance_rescale: float = 0.0) -> None:
+        """The denoising loop (pipeline :492-561) on `latents`, in place: per step, this GPU's windows, then fused_step
+        (after mimo_cfg_rescale when CFG is on and guidance_rescale > 0)."""
         device, dtype = self.device, latents.dtype
         F_, h, w = latents.shape[2:]
         do_cfg = guidance_scale > 1.0
+        # every rank holds the whole clip's prediction here, so the clip-wide statistics need no communication
+        rescaled = torch.empty_like(latents) if do_cfg and guidance_rescale > 0 else None
         rep, nb, single = 2 if do_cfg else 1, len(branches), len(windows) == 1
         den = self.denoising_unet.engine()
         my_windows = plan.windows_of(len(windows)) if plan else list(range(len(windows)))
@@ -626,12 +640,18 @@ class Pose2VideoPipeline:
                         counter[c] = counter[c] + 1
             # the reference divides the window sums by `counter` only inside its guidance branch (pipeline :545-549):
             # without CFG, frames that two windows cover keep the SUM of both predictions - mirrored, not repaired
-            pc, g_, cnt = (noise_pred[1], guidance_scale, counter) if do_cfg else (noise_pred[0], 1.0, None)
+            pu, pc, g_, cnt = (noise_pred[0], noise_pred[1], guidance_scale, counter) if do_cfg else (
+                noise_pred[0], noise_pred[0], 1.0, None)
+            if rescaled is not None:
+                # diffusers' rescale_noise_cfg sits between the guidance line and the step; the step kernels pass a
+                # prediction given as both halves at guidance 1 through unchanged: rnd(v + rnd(1 * rnd(v - v))) = v
+                ops.cfg_rescale(pu, pc, g_, guidance_rescale, out=rescaled, counter=cnt, frame_stride=h * w)
+                pu, pc, g_, cnt = rescaled, rescaled, 1.0, None
             noise = None
             if draws:  # one draw per step, also at the last one where its coefficient is 0 (DDIMScheduler.step [3P])
                 noise = (step_noise[i] if step_noise is not None
                          else torch.randn(tuple(latents.shape), device=device, dtype=dtype))
-            sched.fused_step(i, t, noise_pred[0], pc, latents, g_, eta=eta, noise=noise, history=history, counter=cnt,
+            sched.fused_step(i, t, pu, pc, latents, g_, eta=eta, noise=noise, history=history, counter=cnt,
                              frame_stride=h * w)
             # the reference's inner `for i in range(num_context_batches)` (pipeline :503-510) shadows the step index: its
             # callback test (:556-561) and the index it passes see the LAST CONTEXT BATCH's index, at every step
@@ -662,7 +682,8 @@ class Pose2VideoPipeline:
                  output_type: Optional[str] = "tensor", return_dict: bool = True,
                  callback: Optional[Callable[[int, int, torch.Tensor], None]] = None,
                  callback_steps: Optional[int] = 1, context_schedule="uniform", context_frames=24, context_stride=1,
-                 context_overlap=4, context_batch_size=1, interpolation_factor=1, **kwargs):
+                 context_overlap=4, context_batch_size=1, interpolation_factor=1, guidance_rescale: float = 0.0,
+                 **kwargs):
         device = self.device
         if device.type != "cuda":
             raise MimoError("Pose2VideoPipeline needs its models on a CUDA (sm_90a) device: no CPU fallback")
@@ -671,6 +692,7 @@ class Pose2VideoPipeline:
                                       "reference's shipped configuration")
         if eta < 0:
             raise ValueError(f"eta={eta}: DDIM's eta is >= 0 (0 deterministic, 1 DDPM-like)")
+        self._check_guidance_rescale(guidance_rescale)
         self._interpolation_method(interpolation_factor, video_length)  # before any work is done
         dtype = self.denoising_unet.dtype
         self.latent_levels(width, height)  # refuses only images smaller than one latent pixel
@@ -681,7 +703,7 @@ class Pose2VideoPipeline:
         self.io_bytes["h2d"] = sum(v.numel() * v.element_size() for v in host.values())
         out = self.sample_tensors(dev_in, num_inference_steps, guidance_scale, context_schedule, context_frames,
                                   context_stride, context_overlap, callback, callback_steps, eta=eta,
-                                  interpolation_factor=interpolation_factor)
+                                  interpolation_factor=interpolation_factor, guidance_rescale=guidance_rescale)
         vid = out["videos"].float()  # :124-126 "always cast to float32": exact, and 20 ms cheaper here than on one host core
         host_vid = torch.empty(vid.shape, dtype=torch.float32, pin_memory=True)
         host_vid.copy_(vid, non_blocking=True)  # one D2H of the finished clip, into pinned memory

@@ -210,6 +210,14 @@ class CfgMultistepParams(C.Structure):
     ]
 
 
+class CfgRescaleParams(C.Structure):
+    _fields_ = [
+        ("pred_uncond", C.c_void_p), ("pred_cond", C.c_void_p), ("counter", C.c_void_p), ("frame_stride", C.c_int64),
+        ("out", C.c_void_p), ("count", C.c_int64), ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64),
+        ("phi", C.c_double), ("guidance", C.c_float), ("dtype", C.c_int32),
+    ]
+
+
 # every symbol include/mimo_b200.h declares: name -> (restype, argtypes)
 _VP, _I32, _I64, _F = C.c_void_p, C.c_int32, C.c_int64, C.c_float
 SYMBOLS = {
@@ -256,6 +264,8 @@ SYMBOLS = {
     "mimo_cfg_ddim_step_noise": (C.c_int, [_VP, _VP, _VP, _I64, _VP, _I64, _F, _F, _F, _F, _F, _VP, _F, _I32, _VP]),
     "mimo_interpolate_frames": (C.c_int, [_VP, _VP, _I32, _I64, _I32, _I32, _I32, _VP]),
     "mimo_cfg_multistep": (C.c_int, [C.POINTER(CfgMultistepParams), _VP]),
+    "mimo_cfg_rescale": (C.c_int, [C.POINTER(CfgRescaleParams), _VP]),
+    "mimo_cfg_rescale_workspace_bytes": (C.c_int64, [C.POINTER(CfgRescaleParams)]),
 }
 # test hook, not part of the public header
 _DEBUG_SYMBOLS = {"mimo_debug_pdl": (C.c_int, [C.c_int]), "mimo_debug_splitk": (C.c_int, [C.c_int]),
@@ -282,7 +292,7 @@ def load() -> C.CDLL:
     for which, st in enumerate((Epilogue, GemmParams, Conv3x3Params, GroupNormParams, AttnParams, AttnTemporalParams,
                              ExchangeParams, CfgMultistepParams, GroupNormWindowParams, GemmE4m3Params,
                              GroupNormE4m3Params, Conv3x3E4m3Params, GemmE4m3GegluE4m3Params,
-                             GemmE4m3BlockscaledParams)):
+                             GemmE4m3BlockscaledParams, CfgRescaleParams)):
         if lib.mimo_abi_sizeof(which) != C.sizeof(st):
             raise MimoError(f"ABI mismatch: {st.__name__} is {C.sizeof(st)} bytes in lib.py but "
                             f"{lib.mimo_abi_sizeof(which)} in {LIB_PATH.name}; rebuild the library")

@@ -748,6 +748,30 @@ def cfg_multistep(pred_uncond: torch.Tensor, pred_cond: torch.Tensor, latents: t
     return latents
 
 
+def cfg_rescale(pred_uncond: torch.Tensor, pred_cond: torch.Tensor, guidance: float, phi: float,
+                out: Optional[torch.Tensor] = None, counter: Optional[torch.Tensor] = None,
+                frame_stride: int = 0) -> torch.Tensor:
+    """Rescaled CFG (guidance_rescale = phi): the guided prediction of the two (window-summed) halves, as cfg_ddim_step
+    forms it, rescaled by std(text) / std(cfg) over the whole tensor and mixed with weight phi, written to `out`
+    (allocated when None). Feed the step kernels (out, out, guidance 1.0, no counter) afterwards."""
+    assert pred_uncond.is_contiguous() and pred_cond.is_contiguous() and pred_cond.dtype == pred_uncond.dtype
+    assert pred_cond.numel() == pred_uncond.numel()
+    if out is None:
+        out = torch.empty_like(pred_cond)
+    assert out.is_contiguous() and out.dtype == pred_cond.dtype and out.numel() == pred_cond.numel()
+    p = L.CfgRescaleParams(pred_uncond=_ptr(pred_uncond), pred_cond=_ptr(pred_cond), counter=_ptr(counter),
+                           frame_stride=int(frame_stride), out=_ptr(out), count=out.numel(), phi=float(phi),
+                           guidance=float(guidance), dtype=_dt(out))
+    need = L.load().mimo_cfg_rescale_workspace_bytes(C.byref(p))
+    if need < 0:
+        L.check(int(need), "mimo_cfg_rescale_workspace_bytes")
+    ws = torch.empty(((need + 7) // 8,), dtype=torch.float64, device=out.device)
+    p.workspace, p.workspace_bytes = _ptr(ws), ws.numel() * 8
+    with _Call("cfg_rescale", 2, 0.0, float(out.element_size() * 3 * out.numel())):  # algorithmic: two reads, one write
+        L.check(L.load().mimo_cfg_rescale(C.byref(p), _stream()), "mimo_cfg_rescale")
+    return out
+
+
 INTERP_LINEAR, INTERP_SLERP = 0, 1
 
 
