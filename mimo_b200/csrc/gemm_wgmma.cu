@@ -30,6 +30,9 @@
 
 #include <cudaTypedefs.h>
 
+#include <cstdio>
+#include <type_traits>
+
 #include "../../include/mimo_b200.h"
 #include "host_util.h"
 #include "ptx.cuh"
@@ -95,12 +98,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
                   const __grid_constant__ CUtensorMap tmRes, int M, int N, int num_m_tiles, int num_n_tiles,
                   int num_k_blocks, ConvGeom g, EpiArgs ep) {
   constexpr bool kE4m3 = false, kImgScale = false;
-  constexpr const float* a_scale = nullptr;
-  constexpr const float* w_scale = nullptr;
+  [[maybe_unused]] constexpr const float* a_scale = nullptr;
+  [[maybe_unused]] constexpr const float* w_scale = nullptr;
   constexpr bool kOutE4m3 = false, kBlockScale = false;
-  constexpr float* out_scale = nullptr;
-  constexpr long long ld_scale = 0;
-  const CUtensorMap& tmAS = tmA0;
+  [[maybe_unused]] constexpr float* out_scale = nullptr;
+  [[maybe_unused]] constexpr long long ld_scale = 0;
+  [[maybe_unused]] const CUtensorMap& tmAS = tmA0;
 #include "gemm_wgmma_body.cuh"
 }
 
@@ -115,9 +118,9 @@ gemm_e4m3_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
                  const float* __restrict__ w_scale) {
   constexpr bool kE4m3 = true, kImgScale = false;
   constexpr bool kOutE4m3 = false, kBlockScale = false;
-  constexpr float* out_scale = nullptr;
-  constexpr long long ld_scale = 0;
-  const CUtensorMap& tmAS = tmA0;
+  [[maybe_unused]] constexpr float* out_scale = nullptr;
+  [[maybe_unused]] constexpr long long ld_scale = 0;
+  [[maybe_unused]] const CUtensorMap& tmAS = tmA0;
 #include "gemm_wgmma_body.cuh"
 }
 
@@ -132,9 +135,9 @@ conv_e4m3_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
                  const float* __restrict__ w_scale) {
   constexpr bool kE4m3 = true, kImgScale = true;
   constexpr bool kOutE4m3 = false, kBlockScale = false;
-  constexpr float* out_scale = nullptr;
-  constexpr long long ld_scale = 0;
-  const CUtensorMap& tmAS = tmA0;
+  [[maybe_unused]] constexpr float* out_scale = nullptr;
+  [[maybe_unused]] constexpr long long ld_scale = 0;
+  [[maybe_unused]] const CUtensorMap& tmAS = tmA0;
 #include "gemm_wgmma_body.cuh"
 }
 
@@ -150,7 +153,7 @@ gemm_e4m3_geglu_e4m3_kernel(const __grid_constant__ CUtensorMap tmA0, const __gr
   constexpr int BN = 256;
   constexpr bool kRes = false;
   constexpr bool kE4m3 = true, kImgScale = false, kOutE4m3 = true, kBlockScale = false;
-  const CUtensorMap& tmAS = tmA0;
+  [[maybe_unused]] const CUtensorMap& tmAS = tmA0;
 #include "gemm_wgmma_body.cuh"
 }
 
@@ -164,9 +167,9 @@ gemm_blockscaled_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_c
                         int N, int num_m_tiles, int num_n_tiles, int num_k_blocks, ConvGeom g, EpiArgs ep,
                         const float* __restrict__ w_scale) {
   constexpr bool kE4m3 = true, kImgScale = false, kOutE4m3 = false, kBlockScale = true;
-  constexpr const float* a_scale = nullptr;
-  constexpr float* out_scale = nullptr;
-  constexpr long long ld_scale = 0;
+  [[maybe_unused]] constexpr const float* a_scale = nullptr;
+  [[maybe_unused]] constexpr float* out_scale = nullptr;
+  [[maybe_unused]] constexpr long long ld_scale = 0;
 #include "gemm_wgmma_body.cuh"
 }
 
@@ -236,66 +239,39 @@ splitk_reduce_kernel(const float* __restrict__ part, int splits, long long M, in
   *reinterpret_cast<uint4*>(static_cast<T*>(out) + row * ldo + col) = o;
 }
 
-// Split-K decision: only when the output tiles would leave more than half of the SMs idle AND every split still gets a
-// long K range (>= 16 K blocks = 1024): the deep, small-M convolutions / FF projections of the 8x8 and 16x16 levels when
-// the clip's frames are spread over several GPUs. Returns the number of splits (1 = off).
-static int pick_splits(long long tiles, int nkb, long long M, int N, int64_t ws_bytes) {
-  if (tiles * 2 > num_sms() || nkb < 32) return 1;
-  long long s = num_sms() / tiles;
-  if (s > nkb / 16) s = nkb / 16;
-  if (s > 16) s = 16;
-  while (s > 1 && s * M * N * 4 > ws_bytes) --s;
-  return s < 2 ? 1 : static_cast<int>(s);
+// Runtime -> compile-time selection: f(std::true_type{}) if b, else f(std::false_type{})
+template <class F>
+static auto with_bool(bool b, F&& f) {
+  return b ? f(std::true_type{}) : f(std::false_type{});
 }
 
-struct Maps {
-  CUtensorMap a0, a1, b, out, res;
+// Errors that name a kernel family: `fmt` holds one %s for `who`; an ARG error unless a CUDA error `e` is given
+static int family_error(const char* fmt, const char* who, cudaError_t e = cudaSuccess) {
+  char msg[128];
+  snprintf(msg, sizeof(msg), fmt, who);
+  return e == cudaSuccess ? set_error(MIMO_ERR_ARG, msg) : set_cuda_error(msg, e);
+}
+
+// The tile widths (BN) a kernel family is instantiated at, widest first (pick_bn's tie-break reads them in this order).
+// dispatch() calls f(std::integral_constant<int, BN>, kBf16, kRes) (the last two std::bool_constants) for the runtime
+// width `bn`, dtype and residual flag, and refuses a width that is not in the list.
+template <int... BNs>
+struct TileWidths {
+  static constexpr int kList[sizeof...(BNs)] = {BNs...};
+  static constexpr bool has(int bn) { return ((bn == BNs) || ...); }
+  template <class F>
+  static int dispatch(const char* who, int bn, int dtype, bool res, F&& f) {
+    int rc = MIMO_OK;
+    auto at = [&](auto kBN) {
+      if (bn != kBN) return false;
+      rc = with_bool(dtype == MIMO_BF16,
+                     [&](auto kBf16) { return with_bool(res, [&](auto kRes) { return f(kBN, kBf16, kRes); }); });
+      return true;
+    };
+    if ((at(std::integral_constant<int, BNs>{}) || ...)) return rc;
+    return family_error("%s: unsupported BN", who);
+  }
 };
-
-template <int BN, bool kBf16, bool kRes>
-static int launch_cfg(const Maps& m, int M, int N, int mt, int nt, int nkb, const ConvGeom& g, const EpiArgs& ep,
-                      cudaStream_t st) {
-  using Cfg = GemmCfg<BN, kRes>;
-  auto kern = gemm_wgmma_kernel<BN, kBf16, kRes>;
-  static bool attr_done = false;  // per instantiation
-  if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
-    if (e != cudaSuccess) return set_cuda_error("cudaFuncSetAttribute(gemm)", e);
-    attr_done = true;
-  }
-  const int tiles = mt * nt;
-  const int grid = tiles < num_sms() ? tiles : num_sms();
-  cudaError_t e = launch_k(kern, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, st, m.a0, m.a1, m.b, m.out, m.res, M, N, mt,
-                           nt, nkb, g, ep);
-  if (e == cudaSuccess) e = cudaGetLastError();
-  if (e != cudaSuccess) return set_cuda_error("gemm launch", e);
-  return MIMO_OK;
-}
-
-template <bool kBf16>
-static int launch_bn(int bn, bool res, const Maps& m, int M, int N, int mt, int nt, int nkb, const ConvGeom& g,
-                     const EpiArgs& ep, cudaStream_t st) {
-  switch (bn) {
-    case 64:
-      return res ? launch_cfg<64, kBf16, true>(m, M, N, mt, nt, nkb, g, ep, st)
-                 : launch_cfg<64, kBf16, false>(m, M, N, mt, nt, nkb, g, ep, st);
-    case 128:
-      return res ? launch_cfg<128, kBf16, true>(m, M, N, mt, nt, nkb, g, ep, st)
-                 : launch_cfg<128, kBf16, false>(m, M, N, mt, nt, nkb, g, ep, st);
-    case 160:
-      return res ? launch_cfg<160, kBf16, true>(m, M, N, mt, nt, nkb, g, ep, st)
-                 : launch_cfg<160, kBf16, false>(m, M, N, mt, nt, nkb, g, ep, st);
-    case 192:
-      return res ? launch_cfg<192, kBf16, true>(m, M, N, mt, nt, nkb, g, ep, st)
-                 : launch_cfg<192, kBf16, false>(m, M, N, mt, nt, nkb, g, ep, st);
-    case 256:
-      return res ? launch_cfg<256, kBf16, true>(m, M, N, mt, nt, nkb, g, ep, st)
-                 : launch_cfg<256, kBf16, false>(m, M, N, mt, nt, nkb, g, ep, st);
-  }
-  return set_error(MIMO_ERR_ARG, "gemm: unsupported BN");
-}
-
-int pick_bn(int N, bool geglu, long long m_tiles);
 
 // ptxas (CUDA 12.9, -O3), per thread at the 168-register cap of 320 threads:
 //   gemm_e4m3_kernel<192, *, *>: 144-155 registers, no spills
@@ -308,59 +284,44 @@ int pick_bn(int N, bool geglu, long long m_tiles);
 //     spill-free kernels here all have)
 //   gemm_blockscaled_kernel<64, *, *>: 91 registers, no spills; <128, *, *>: 146 registers, no spills (two BN / 2
 //     accumulators per thread: the running sum and the K block's own)
-// e4m3 tile widths (gemm_e4m3_kernel instantiations): 192 and 256 are the widths pick_bn gives the LN-fed GEMMs of the
-// UNet (q|k|v N = 3 C: 960 / 1920 -> 192, 3840 -> 256; GEGLU N = 8 C -> 256).
-template <bool kBf16>
-static int launch_e4m3(int bn, bool res, const Maps& m, int M, int N, int mt, int nt, int nkb, const ConvGeom& g,
-                       const EpiArgs& ep, const float* a_scale, const float* w_scale, cudaStream_t st) {
-  auto run = [&](auto kern, int smem) -> int {
-    static bool attr_done[2][2][2] = {};  // [bn == 256][kBf16][res]
-    bool& done = attr_done[bn == 256][kBf16][res];
-    if (!done) {
-      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-      if (e != cudaSuccess) return set_cuda_error("cudaFuncSetAttribute(gemm_e4m3)", e);
-      done = true;
-    }
-    const int tiles = mt * nt;
-    const int grid = tiles < num_sms() ? tiles : num_sms();
-    cudaError_t e = launch_k(kern, dim3(grid), dim3(kGemmThreads), smem, st, m.a0, m.a1, m.b, m.out, m.res, M, N, mt, nt,
-                             nkb, g, ep, a_scale, w_scale);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e != cudaSuccess) return set_cuda_error("gemm_e4m3 launch", e);
-    return MIMO_OK;
-  };
-  if (bn == 192)
-    return res ? run(gemm_e4m3_kernel<192, kBf16, true>, GemmCfg<192, true, true>::kSmemBytes)
-               : run(gemm_e4m3_kernel<192, kBf16, false>, GemmCfg<192, false, true>::kSmemBytes);
-  if (bn == 256)
-    return res ? run(gemm_e4m3_kernel<256, kBf16, true>, GemmCfg<256, true, true>::kSmemBytes)
-               : run(gemm_e4m3_kernel<256, kBf16, false>, GemmCfg<256, false, true>::kSmemBytes);
-  return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3: unsupported BN");
-}
+// e4m3 tile widths: 192 and 256 are the widths pick_bn gives the LN-fed GEMMs of the UNet (q|k|v N = 3 C: 960 / 1920 ->
+// 192, 3840 -> 256; GEGLU N = 8 C -> 256).
+using Widths16 = TileWidths<256, 192, 160, 128, 64>;  // gemm_wgmma_kernel
+using WidthsE4m3 = TileWidths<256, 192>;              // gemm_e4m3_kernel
+using WidthsConvE4m3 = TileWidths<256, 160>;          // conv_e4m3_kernel (choice: pick_bn_conv_e4m3)
+using WidthsGegluE4m3 = TileWidths<256>;              // gemm_e4m3_geglu_e4m3_kernel, which takes no residual
+using WidthsBlockScaled = TileWidths<128, 64>;        // gemm_blockscaled_kernel (choice: pick_bn_blockscaled)
 
-// e4m3 tile width: pick_bn's rule over the instantiated widths {256, 192} - least padded columns, then the wider; GEGLU
-// takes pick_bn's own width (it fixes the weight packing, mimo_gemm_geglu_granule) and must be one of them.
-static int pick_bn_e4m3(int N, bool geglu) {
-  if (geglu) return pick_bn(N, true, 1 << 20);
-  const int pad256 = (N + 255) / 256 * 256 - N, pad192 = (N + 191) / 192 * 192 - N;
-  return pad192 < pad256 ? 192 : 256;
+// One launch of a persistent GEMM / conv kernel: min(tiles, SMs) CTAs of kGemmThreads with kSmem bytes of dynamic shared
+// memory (the attribute is set on the first launch of each kernel). `who` names the kernel family in error messages.
+template <auto kKern, int kSmem, class... A>
+static int launch_gemm_kernel(const char* who, int tiles, cudaStream_t st, A... args) {
+  static bool attr_done = false;  // per instantiation
+  if (!attr_done) {
+    const cudaError_t e = cudaFuncSetAttribute(kKern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
+    if (e != cudaSuccess) return family_error("cudaFuncSetAttribute(%s)", who, e);
+    attr_done = true;
+  }
+  const int grid = tiles < num_sms() ? tiles : num_sms();
+  cudaError_t e = launch_k(kKern, dim3(grid), dim3(kGemmThreads), kSmem, st, args...);
+  if (e == cudaSuccess) e = cudaGetLastError();
+  if (e != cudaSuccess) return family_error("%s launch", who, e);
+  return MIMO_OK;
 }
 
 static int g_force_bn = 0;
 
 // Tile-width choice: least padded columns first, then the widest tile (fewer A re-reads, higher MMA N).
-int pick_bn(int N, bool geglu, long long m_tiles) {
+static int pick_bn(int N, bool geglu, long long m_tiles) {
   if (g_force_bn) return g_force_bn;
   if (geglu) {
     if (N % 256 == 0) return 256;
     if (N % 128 == 0) return 128;
     return 64;
   }
-  const int cands[5] = {256, 192, 160, 128, 64};
   int best = 64;
   double best_eff = -1.0;
-  for (int i = 0; i < 5; ++i) {
-    const int bn = cands[i];
+  for (const int bn : Widths16::kList) {
     const int nt = (N + bn - 1) / bn;
     double eff = static_cast<double>(N) / (static_cast<double>(nt) * bn);
     // small problems: prefer enough tiles to occupy the machine
@@ -372,6 +333,53 @@ int pick_bn(int N, bool geglu, long long m_tiles) {
     }
   }
   return best;
+}
+
+// e4m3 tile width: pick_bn's rule over the instantiated widths {256, 192} - least padded columns, then the wider; GEGLU
+// takes pick_bn's own width (it fixes the weight packing, mimo_gemm_geglu_granule) and must be one of them.
+static int pick_bn_e4m3(int N, bool geglu) {
+  if (geglu) return pick_bn(N, true, 1 << 20);
+  const int pad256 = (N + 255) / 256 * 256 - N, pad192 = (N + 191) / 192 * 192 - N;
+  return pad192 < pad256 ? 192 : 256;
+}
+
+// e4m3 conv tile widths (conv_e4m3_kernel instantiations): 160 divides every ResBlock width (320, 640, 1280), 256 divides
+// 1280. At 1280 BN 256 spills (ptxas report above) and 160 does not; measured on an H100 SXM (700 W) at the 48 images of
+// the 512 x 512 CFG window, 256 was faster where its tiles fit one wave and 160's did not (8 x 8: 66 / 68 / 123 us
+// against 83 / 85 / 152 us), and at 16 x 16 the two were within 8 % either way (scripts/fp8_conv_bench.py). So: 256 when
+// that saves a wave, else the least padded width, 160 on a tie.
+static int pick_bn_conv_e4m3(int N, long long m_tiles) {
+  if (g_force_bn) return g_force_bn;
+  const long long t256 = m_tiles * ((N + 255) / 256), t160 = m_tiles * ((N + 159) / 160);
+  if (N % 256 == 0 && t256 <= num_sms() && t160 > num_sms()) return 256;
+  const int pad256 = (N + 255) / 256 * 256 - N, pad160 = (N + 159) / 160 * 160 - N;
+  return pad256 < pad160 ? 256 : 160;
+}
+
+// block-scaled tile widths (gemm_blockscaled_kernel instantiations): the per-block accumulator doubles the accumulator
+// registers, so 64 and 128 (ptxas report above). Measured on an H100 SXM (700 W) at the FF-out shapes of the 512 x 512
+// CFG window (scripts/fp8_ff_bench.py), 128 was faster at every width, even at N = 320 where it pads to 384 columns
+// (290 against 302 us at 64 x 64: 3 column tiles read each A tile 3 times instead of 5): 128, and 64 only for N <= 64.
+static int pick_bn_blockscaled(int N) {
+  if (g_force_bn) return g_force_bn;
+  return N <= 64 ? 64 : 128;
+}
+
+// Split-K decision: only when the output tiles would leave more than half of the SMs idle AND every split still gets a
+// long K range (>= 16 K blocks = 1024): the deep, small-M convolutions / FF projections of the 8x8 and 16x16 levels when
+// the clip's frames are spread over several GPUs. Returns the number of splits (1 = off); a split problem takes the tile
+// width a large problem would get, written to `bn`.
+static int pick_splits(int& bn, int N, int mt, int nkb, long long M, int64_t ws_bytes) {
+  const int bn_wide = pick_bn(N, false, 1 << 20);
+  const long long tiles = static_cast<long long>(mt) * ((N + bn_wide - 1) / bn_wide);
+  if (tiles * 2 > num_sms() || nkb < 32) return 1;
+  long long s = num_sms() / tiles;
+  if (s > nkb / 16) s = nkb / 16;
+  if (s > 16) s = 16;
+  while (s > 1 && s * M * N * 4 > ws_bytes) --s;
+  if (s < 2) return 1;
+  bn = bn_wide;
+  return static_cast<int>(s);
 }
 
 static EpiArgs make_epi(const mimo_epilogue& e, int N) {
@@ -408,6 +416,127 @@ static int launch_reduce(int dtype, const float* part, int splits, long long M, 
   return MIMO_OK;
 }
 
+// Geometry of plain GEMM rows: K blocks kb0 of source 0 (K = c0 elements) and kb1 of source 1, 128 x 32 output chunks,
+// no split
+static ConvGeom gemm_rows(int c0, int kb0, int kb1 = 0) {
+  ConvGeom g = {};
+  g.c0 = c0;
+  g.kb0 = kb0;
+  g.kb1 = kb1;
+  g.chunk_bytes = kChunk;
+  g.splits = 1;
+  g.kb_split = kb0 + kb1;
+  return g;
+}
+
+// Conv geometry: `ntaps` taps at input offsets (tdx, tdy) over [n, h, w] images of c0 (+ c1) channels, in K blocks of kc
+// channels of esz bytes each, and the {TW, TH, TN} output footprint of a 128-row tile; no split, so kb_split holds all
+// ntaps * (kb0 + kb1) K blocks. Returns the M tiles.
+static int conv_geom(ConvGeom& g, int n, int h, int w, int c0, int c1, int kc, int esz, int ntaps,
+                     const signed char* tdx, const signed char* tdy) {
+  g = {};
+  g.conv = 1;
+  g.H = h;
+  g.W = w;
+  g.NI = n;
+  g.TW = w < BM ? w : BM;
+  g.TH = BM / g.TW;
+  if (g.TH > h) g.TH = h;
+  if (g.TH < 1) g.TH = 1;
+  g.TN = BM / (g.TW * g.TH);
+  if (g.TN > n) g.TN = n;
+  if (g.TN < 1) g.TN = 1;
+  if (g.TN > 1 && g.TH != h) g.TN = 1;  // several images per tile only when a tile spans whole images
+  g.tiles_w = (w + g.TW - 1) / g.TW;
+  g.tiles_h = (h + g.TH - 1) / g.TH;
+  g.ctot = c0 + c1;
+  g.c0 = c0;
+  g.kb0 = (c0 + kc - 1) / kc;
+  g.kb1 = (c1 + kc - 1) / kc;
+  const int pixels = g.TW * g.TH * g.TN;
+  g.a_bytes = pixels * kc * esz;
+  g.chunk_bytes = pixels * 64;
+  g.splits = 1;
+  g.kb_split = ntaps * (g.kb0 + g.kb1);
+  g.ntaps = ntaps;
+  for (int t = 0; t < 9; ++t) {
+    g.tdx[t] = t < ntaps ? tdx[t] : 0;
+    g.tdy[t] = t < ntaps ? tdy[t] : 0;
+  }
+  return g.tiles_w * g.tiles_h * ((n + g.TN - 1) / g.TN);
+}
+
+constexpr signed char kTap3x3Dx[9] = {-1, 0, 1, -1, 0, 1, -1, 0, 1};
+constexpr signed char kTap3x3Dy[9] = {-1, -1, -1, 0, 0, 0, 1, 1, 1};
+
+struct Maps {
+  CUtensorMap a0, a1, b, out, res;
+};
+
+// 2-D map over `rows` rows of `cols` elements (`dtype`: 16-bit, or kTmapU8) that start `pitch` bytes apart
+static int rows_map(CUtensorMap* tm, int dtype, const void* base, uint64_t cols, uint64_t rows, uint64_t pitch,
+                    uint32_t box_cols, uint32_t box_rows, int swizzle = 128) {
+  const uint64_t dim[2] = {cols, rows};
+  const uint64_t str[1] = {pitch};
+  const uint32_t box[2] = {box_cols, box_rows};
+  return encode_tmap(tm, dtype, 2, base, dim, str, box, swizzle);
+}
+
+// 4-D map over the NHWC images of g, `c` channels of `dtype` each: pixel (n, y, x) at
+// base + ((n * s H + y s) * s W + x s) * pitch elements, i.e. a stride-s view of s times larger images when s > 1. Box
+// {box_c, TW, TH, TN}.
+static int nhwc_map(CUtensorMap* tm, int dtype, const void* base, const ConvGeom& g, int c, long long pitch,
+                    uint32_t box_c, int swizzle, int s = 1) {
+  const uint64_t dim[4] = {static_cast<uint64_t>(c), static_cast<uint64_t>(g.W), static_cast<uint64_t>(g.H),
+                           static_cast<uint64_t>(g.NI)};
+  uint64_t str[3];
+  str[0] = static_cast<uint64_t>(s) * pitch * (dtype == kTmapU8 ? 1 : 2);
+  str[1] = static_cast<uint64_t>(s) * g.W * str[0];
+  str[2] = static_cast<uint64_t>(g.H) * str[1];
+  const uint32_t box[4] = {box_c, static_cast<uint32_t>(g.TW), static_cast<uint32_t>(g.TH), static_cast<uint32_t>(g.TN)};
+  return encode_tmap(tm, dtype, 4, base, dim, str, box, swizzle);
+}
+
+// 16-bit output and (if `residual`) residual maps of GEMM rows: 128-row x 32-column boxes, 64-byte swizzle. Without a
+// residual m.res repeats m.out; the kernel does not read it.
+static int out_maps_rows(Maps& m, int dtype, void* out, long long ldo, const void* residual, long long ld_res, int cols,
+                         int rows) {
+  if (int rc = rows_map(&m.out, dtype, out, cols, rows, ldo * 2, 32, BM, 64)) return rc;
+  m.res = m.out;
+  return residual ? rows_map(&m.res, dtype, residual, cols, rows, ld_res * 2, 32, BM, 64) : MIMO_OK;
+}
+
+// The same for conv outputs: {32, TW, TH, TN} boxes; the output may be a stride-s view (nhwc_map), the residual is dense
+static int out_maps_nhwc(Maps& m, int dtype, const ConvGeom& g, void* out, long long ldo, int s, const void* residual,
+                         long long ld_res, int cout) {
+  if (int rc = nhwc_map(&m.out, dtype, out, g, cout, ldo, 32, 64, s)) return rc;
+  m.res = m.out;
+  return residual ? nhwc_map(&m.res, dtype, residual, g, cout, ld_res, 32, 64) : MIMO_OK;
+}
+
+// The 16-bit kernel (mimo_gemm, mimo_conv3x3, mimo_conv_up2x) at tile width bn. With splits > 1 the kernel writes each
+// split's fp32 partial sums to `workspace` with its epilogue neutralised, and splitk_reduce_kernel then applies the whole
+// epilogue `e` to `out`.
+static int launch_16bit(int dtype, int bn, bool res, int splits, const Maps& m, int M, int N, int mt, int nkb,
+                        ConvGeom g, const mimo_epilogue& e, void* workspace, void* out, long long ldo, cudaStream_t st) {
+  g.splits = splits;
+  g.kb_split = (nkb + splits - 1) / splits;
+  EpiArgs ep = make_epi(e, N);
+  if (splits > 1) {
+    ep.bias = ep.rowvec = nullptr;
+    ep.act = MIMO_ACT_NONE;
+    ep.scale = 1.0f;
+    ep.partial = static_cast<float*>(workspace);
+  }
+  const int nt = (N + bn - 1) / bn;
+  const int rc = Widths16::dispatch("gemm", bn, dtype, res, [&](auto kBN, auto kBf16, auto kRes) {
+    return launch_gemm_kernel<gemm_wgmma_kernel<kBN, kBf16, kRes>, GemmCfg<kBN, kRes>::kSmemBytes>(
+        "gemm", mt * nt, st, m.a0, m.a1, m.b, m.out, m.res, M, N, mt, nt, nkb, g, ep);
+  });
+  if (rc || splits == 1) return rc;
+  return launch_reduce(dtype, ep.partial, splits, M, N, e, out, ldo, st);
+}
+
 }  // namespace mimo
 
 using namespace mimo;
@@ -433,70 +562,32 @@ extern "C" int mimo_gemm(const mimo_gemm_params* p, void* stream) {
   const bool geglu = p->ep.act == MIMO_ACT_GEGLU;
   if (geglu && (p->ep.residual || p->ep.rowvec))
     return set_error(MIMO_ERR_ARG, "mimo_gemm: GEGLU takes neither a residual nor a row vector");
-  if (int rc = ensure_device()) return rc;
-  const int mt = (p->M + BM - 1) / BM;
   const int K1 = p->a1 ? p->K1 : 0;
   if (K1 < 0 || (K1 % 8) || (p->a1 && (p->lda1 % 8))) return set_error(MIMO_ERR_ARG, "mimo_gemm: K1/lda1 % 8 != 0");
+  // (GEGLU's width does not depend on the SM count, and a GEGLU GEMM is never split)
+  if (geglu && (p->N % pick_bn(p->N, true, 0))) return set_error(MIMO_ERR_ARG, "mimo_gemm: GEGLU needs N % tile == 0");
+  if (int rc = ensure_device()) return rc;
+  const int mt = (p->M + BM - 1) / BM;
   const int kb0 = (p->K + BK - 1) / BK;
   const int kb1 = (K1 + BK - 1) / BK;
   const int nkb = kb0 + kb1;
   int bn = pick_bn(p->N, geglu, mt);
-  int splits = 1;
-  if (!geglu && g_splitk && p->workspace && !g_force_bn) {
-    const int bn_wide = pick_bn(p->N, false, 1 << 20);  // the tile width a large problem would get
-    splits = pick_splits(static_cast<long long>(mt) * ((p->N + bn_wide - 1) / bn_wide), nkb, p->M, p->N, p->workspace_bytes);
-    if (splits > 1) bn = bn_wide;
-  }
-  if (geglu && (p->N % bn)) return set_error(MIMO_ERR_ARG, "mimo_gemm: GEGLU needs N % tile == 0");
-  const int nt = (p->N + bn - 1) / bn;
-  const bool res = p->ep.residual != nullptr && !geglu && splits == 1;
+  const int splits = !geglu && g_splitk && p->workspace && !g_force_bn
+                         ? pick_splits(bn, p->N, mt, nkb, p->M, p->workspace_bytes)
+                         : 1;
+  const bool res = p->ep.residual != nullptr && splits == 1;
 
   Maps m;
-  const uint64_t adim[2] = {static_cast<uint64_t>(p->K), static_cast<uint64_t>(p->M)};
-  const uint64_t astr[1] = {static_cast<uint64_t>(p->lda) * 2};
-  const uint32_t abox[2] = {BK, BM};
-  if (int rc = encode_tmap(&m.a0, p->dtype, 2, p->a, adim, astr, abox)) return rc;
+  if (int rc = rows_map(&m.a0, p->dtype, p->a, p->K, p->M, p->lda * 2, BK, BM)) return rc;
   m.a1 = m.a0;
-  if (K1) {
-    const uint64_t a1dim[2] = {static_cast<uint64_t>(K1), static_cast<uint64_t>(p->M)};
-    const uint64_t a1str[1] = {static_cast<uint64_t>(p->lda1) * 2};
-    if (int rc = encode_tmap(&m.a1, p->dtype, 2, p->a1, a1dim, a1str, abox)) return rc;
-  }
-  const uint64_t bdim[2] = {static_cast<uint64_t>(p->K + K1), static_cast<uint64_t>(p->N)};
-  const uint64_t bstr[1] = {static_cast<uint64_t>(p->ldw) * 2};
-  const uint32_t bbox[2] = {BK, static_cast<uint32_t>(bn)};
-  if (int rc = encode_tmap(&m.b, p->dtype, 2, p->w, bdim, bstr, bbox)) return rc;
-  // output / residual: 128-row x 32-column boxes, 64-byte swizzle
+  if (K1)
+    if (int rc = rows_map(&m.a1, p->dtype, p->a1, K1, p->M, p->lda1 * 2, BK, BM)) return rc;
+  if (int rc = rows_map(&m.b, p->dtype, p->w, p->K + K1, p->N, p->ldw * 2, BK, bn)) return rc;
   const int n_out = geglu ? p->N / 2 : p->N;
-  const uint64_t odim[2] = {static_cast<uint64_t>(n_out), static_cast<uint64_t>(p->M)};
-  const uint64_t ostr[1] = {static_cast<uint64_t>(p->ldo) * 2};
-  const uint32_t obox[2] = {32, BM};
-  if (int rc = encode_tmap(&m.out, p->dtype, 2, p->out, odim, ostr, obox, 64)) return rc;
-  m.res = m.out;
-  if (res) {
-    const uint64_t rstr[1] = {static_cast<uint64_t>(p->ep.ld_res) * 2};
-    if (int rc = encode_tmap(&m.res, p->dtype, 2, p->ep.residual, odim, rstr, obox, 64)) return rc;
-  }
-
-  ConvGeom g = {};
-  g.kb0 = kb0;
-  g.kb1 = kb1;
-  g.c0 = p->K;
-  g.chunk_bytes = kChunk;
-  g.splits = splits;
-  g.kb_split = (nkb + splits - 1) / splits;
-  EpiArgs ep = make_epi(p->ep, p->N);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (splits > 1) {
-    ep.bias = ep.rowvec = nullptr;
-    ep.act = MIMO_ACT_NONE;
-    ep.scale = 1.0f;
-    ep.partial = static_cast<float*>(p->workspace);
-  }
-  const int rc = p->dtype == MIMO_BF16 ? launch_bn<true>(bn, res, m, p->M, p->N, mt, nt, nkb, g, ep, st)
-                                       : launch_bn<false>(bn, res, m, p->M, p->N, mt, nt, nkb, g, ep, st);
-  if (rc || splits == 1) return rc;
-  return launch_reduce(p->dtype, ep.partial, splits, p->M, p->N, p->ep, p->out, p->ldo, st);
+  if (int rc = out_maps_rows(m, p->dtype, p->out, p->ldo, res ? p->ep.residual : nullptr, p->ep.ld_res, n_out, p->M))
+    return rc;
+  return launch_16bit(p->dtype, bn, res, splits, m, p->M, p->N, mt, nkb, gemm_rows(p->K, kb0, kb1), p->ep, p->workspace,
+                      p->out, p->ldo, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int mimo_gemm_e4m3(const mimo_gemm_e4m3_params* p, void* stream) {
@@ -516,7 +607,7 @@ extern "C" int mimo_gemm_e4m3(const mimo_gemm_e4m3_params* p, void* stream) {
     return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3: GEGLU takes neither a residual nor a row vector");
   const int bn = pick_bn_e4m3(p->N, geglu);
   if (geglu && (p->N % bn)) return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3: GEGLU needs N % tile == 0");
-  if (bn != 192 && bn != 256) return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3: GEGLU needs N % 256 == 0");
+  if (!WidthsE4m3::has(bn)) return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3: GEGLU needs N % 256 == 0");
   if (int rc = ensure_device()) return rc;
   const int mt = (p->M + BM - 1) / BM;
   const int nt = (p->N + bn - 1) / bn;
@@ -524,136 +615,53 @@ extern "C" int mimo_gemm_e4m3(const mimo_gemm_e4m3_params* p, void* stream) {
   const bool res = p->ep.residual != nullptr && !geglu;
 
   Maps m;
-  const uint64_t adim[2] = {static_cast<uint64_t>(p->K), static_cast<uint64_t>(p->M)};
-  const uint64_t astr[1] = {static_cast<uint64_t>(p->lda)};
-  const uint32_t abox[2] = {2 * BK, BM};
-  if (int rc = encode_tmap(&m.a0, kTmapU8, 2, p->a, adim, astr, abox)) return rc;
+  if (int rc = rows_map(&m.a0, kTmapU8, p->a, p->K, p->M, p->lda, 2 * BK, BM)) return rc;
   m.a1 = m.a0;
-  const uint64_t bdim[2] = {static_cast<uint64_t>(p->K), static_cast<uint64_t>(p->N)};
-  const uint64_t bstr[1] = {static_cast<uint64_t>(p->ldw)};
-  const uint32_t bbox[2] = {2 * BK, static_cast<uint32_t>(bn)};
-  if (int rc = encode_tmap(&m.b, kTmapU8, 2, p->w, bdim, bstr, bbox)) return rc;
+  if (int rc = rows_map(&m.b, kTmapU8, p->w, p->K, p->N, p->ldw, 2 * BK, bn)) return rc;
   const int n_out = geglu ? p->N / 2 : p->N;
-  const uint64_t odim[2] = {static_cast<uint64_t>(n_out), static_cast<uint64_t>(p->M)};
-  const uint64_t ostr[1] = {static_cast<uint64_t>(p->ldo) * 2};
-  const uint32_t obox[2] = {32, BM};
-  if (int rc = encode_tmap(&m.out, p->dtype, 2, p->out, odim, ostr, obox, 64)) return rc;
-  m.res = m.out;
-  if (res) {
-    const uint64_t rstr[1] = {static_cast<uint64_t>(p->ep.ld_res) * 2};
-    if (int rc = encode_tmap(&m.res, p->dtype, 2, p->ep.residual, odim, rstr, obox, 64)) return rc;
-  }
-  ConvGeom g = {};
-  g.kb0 = nkb;
-  g.c0 = p->K;
-  g.chunk_bytes = kChunk;
-  g.splits = 1;
-  g.kb_split = nkb;
+  if (int rc = out_maps_rows(m, p->dtype, p->out, p->ldo, res ? p->ep.residual : nullptr, p->ep.ld_res, n_out, p->M))
+    return rc;
+  const ConvGeom g = gemm_rows(p->K, nkb);
   const EpiArgs ep = make_epi(p->ep, p->N);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  return p->dtype == MIMO_BF16 ? launch_e4m3<true>(bn, res, m, p->M, p->N, mt, nt, nkb, g, ep, p->a_scale, p->w_scale, st)
-                               : launch_e4m3<false>(bn, res, m, p->M, p->N, mt, nt, nkb, g, ep, p->a_scale, p->w_scale, st);
-}
-
-// conv mode and the {TW, TH, TN} output footprint of a 128-row tile over [n, h, w] images; returns the tiles along n
-static int conv_tiles(ConvGeom& g, int n, int h, int w) {
-  g.conv = 1;
-  g.H = h;
-  g.W = w;
-  g.NI = n;
-  g.TW = w < BM ? w : BM;
-  g.TH = BM / g.TW;
-  if (g.TH > h) g.TH = h;
-  if (g.TH < 1) g.TH = 1;
-  g.TN = BM / (g.TW * g.TH);
-  if (g.TN > n) g.TN = n;
-  if (g.TN < 1) g.TN = 1;
-  if (g.TN > 1 && g.TH != h) g.TN = 1;  // several images per tile only when a tile spans whole images
-  g.tiles_w = (w + g.TW - 1) / g.TW;
-  g.tiles_h = (h + g.TH - 1) / g.TH;
-  return (n + g.TN - 1) / g.TN;
+  return WidthsE4m3::dispatch("gemm_e4m3", bn, p->dtype, res, [&](auto kBN, auto kBf16, auto kRes) {
+    return launch_gemm_kernel<gemm_e4m3_kernel<kBN, kBf16, kRes>, GemmCfg<kBN, kRes, true>::kSmemBytes>(
+        "gemm_e4m3", mt * nt, st, m.a0, m.a1, m.b, m.out, m.res, p->M, p->N, mt, nt, nkb, g, ep, p->a_scale, p->w_scale);
+  });
 }
 
 // One implicit-GEMM convolution launch: `ntaps` taps at offsets (tdx, tdy) over the [n, h, w, c] input(s); the output
-// (and residual) pixel (n, y, x) lives at out + ((n * oh + y * sy) * ow + x * sx) * ldo elements, i.e. a strided view of a
-// larger image when (sx, sy) != (1, 1).
+// (and residual) pixel (n, y, x) lives at out + ((n * s h + y s) * s w + x s) * ldo elements, i.e. a strided view of a
+// larger image when s > 1.
 static int conv_launch(const mimo_conv3x3_params* p, const void* w, int ntaps, const signed char* tdx,
-                       const signed char* tdy, void* out, int sx, int sy, int ow, int oh, void* stream) {
+                       const signed char* tdy, void* out, int s, void* stream) {
   const int c1 = p->x1 ? p->c1 : 0;
-  ConvGeom g = {};
-  const int tiles_n = conv_tiles(g, p->n, p->h, p->w_);
-  g.ctot = p->c0 + c1;
-  g.c0 = p->c0;
-  g.kb0 = (p->c0 + BK - 1) / BK;
-  g.kb1 = (c1 + BK - 1) / BK;
-  g.a_bytes = g.TW * g.TH * g.TN * BK * 2;
-  g.chunk_bytes = g.TW * g.TH * g.TN * 64;
-  g.ntaps = ntaps;
-  for (int t = 0; t < 9; ++t) {
-    g.tdx[t] = t < ntaps ? tdx[t] : 0;
-    g.tdy[t] = t < ntaps ? tdy[t] : 0;
-  }
-  const int mt = g.tiles_w * g.tiles_h * tiles_n;
-  const int nkb = ntaps * (g.kb0 + g.kb1);
+  ConvGeom g;
+  const int mt = conv_geom(g, p->n, p->h, p->w_, p->c0, c1, BK, 2, ntaps, tdx, tdy);
+  const int nkb = g.kb_split;
   const long long Mrows = static_cast<long long>(p->n) * p->h * p->w_;
   if (Mrows > 0x7fffffffLL) return set_error(MIMO_ERR_ARG, "mimo_conv: too many pixels");
   int bn = pick_bn(p->cout, false, mt);
-  int splits = 1;
   // split-K needs the dense NHWC output (row = pixel index): not for the strided parity classes of mimo_conv_up2x
-  if (g_splitk && p->workspace && !g_force_bn && sx == 1 && sy == 1 && p->ldo == p->cout) {
-    const int bn_wide = pick_bn(p->cout, false, 1 << 20);
-    splits = pick_splits(static_cast<long long>(mt) * ((p->cout + bn_wide - 1) / bn_wide), nkb, Mrows, p->cout,
-                         p->workspace_bytes);
-    if (splits > 1) bn = bn_wide;
-  }
-  g.splits = splits;
-  g.kb_split = (nkb + splits - 1) / splits;
-  const int nt = (p->cout + bn - 1) / bn;
+  const int splits = g_splitk && p->workspace && !g_force_bn && s == 1 && p->ldo == p->cout
+                         ? pick_splits(bn, p->cout, mt, nkb, Mrows, p->workspace_bytes)
+                         : 1;
   const bool res = p->ep.residual != nullptr && splits == 1;
 
   Maps m;
-  auto nhwc_map = [&](CUtensorMap* tm, const void* base, int c, long long pitch, uint32_t box_c, int swz, int px,
-                      int py, int iw, int ih) {
-    // pixel (n, y, x) at base + ((n * ih + y * py) * iw + x * px) * pitch elements
-    const uint64_t dim[4] = {static_cast<uint64_t>(c), static_cast<uint64_t>(p->w_), static_cast<uint64_t>(p->h),
-                             static_cast<uint64_t>(p->n)};
-    const uint64_t str[3] = {static_cast<uint64_t>(px) * pitch * 2, static_cast<uint64_t>(py) * iw * pitch * 2,
-                             static_cast<uint64_t>(ih) * iw * pitch * 2};
-    const uint32_t box[4] = {box_c, static_cast<uint32_t>(g.TW), static_cast<uint32_t>(g.TH),
-                             static_cast<uint32_t>(g.TN)};
-    return encode_tmap(tm, p->dtype, 4, base, dim, str, box, swz);
-  };
-  if (int rc = nhwc_map(&m.a0, p->x0, p->c0, p->c0, BK, 128, 1, 1, p->w_, p->h)) return rc;
+  if (int rc = nhwc_map(&m.a0, p->dtype, p->x0, g, p->c0, p->c0, BK, 128)) return rc;
   m.a1 = m.a0;
   if (c1)
-    if (int rc = nhwc_map(&m.a1, p->x1, c1, c1, BK, 128, 1, 1, p->w_, p->h)) return rc;
-  {
-    const uint64_t dim[2] = {static_cast<uint64_t>(ntaps) * g.ctot, static_cast<uint64_t>(p->cout)};
-    const uint64_t str[1] = {static_cast<uint64_t>(ntaps) * g.ctot * 2};
-    const uint32_t box[2] = {BK, static_cast<uint32_t>(bn)};
-    if (int rc = encode_tmap(&m.b, p->dtype, 2, w, dim, str, box)) return rc;
-  }
-  if (int rc = nhwc_map(&m.out, out, p->cout, p->ldo, 32, 64, sx, sy, ow, oh)) return rc;
-  m.res = m.out;
-  if (res)
-    if (int rc = nhwc_map(&m.res, p->ep.residual, p->cout, p->ep.ld_res, 32, 64, 1, 1, p->w_, p->h)) return rc;
-
-  EpiArgs ep = make_epi(p->ep, p->cout);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (splits > 1) {
-    ep.bias = ep.rowvec = nullptr;
-    ep.act = MIMO_ACT_NONE;
-    ep.scale = 1.0f;
-    ep.partial = static_cast<float*>(p->workspace);
-  }
-  const int rc = p->dtype == MIMO_BF16
-                     ? launch_bn<true>(bn, res, m, static_cast<int>(Mrows), p->cout, mt, nt, nkb, g, ep, st)
-                     : launch_bn<false>(bn, res, m, static_cast<int>(Mrows), p->cout, mt, nt, nkb, g, ep, st);
-  if (rc || splits == 1) return rc;
-  return launch_reduce(p->dtype, ep.partial, splits, Mrows, p->cout, p->ep, out, p->ldo, st);
+    if (int rc = nhwc_map(&m.a1, p->dtype, p->x1, g, c1, c1, BK, 128)) return rc;
+  const long long kw = static_cast<long long>(ntaps) * g.ctot;  // weight row: [tap][channel]
+  if (int rc = rows_map(&m.b, p->dtype, w, kw, p->cout, kw * 2, BK, bn)) return rc;
+  if (int rc = out_maps_nhwc(m, p->dtype, g, out, p->ldo, s, res ? p->ep.residual : nullptr, p->ep.ld_res, p->cout))
+    return rc;
+  return launch_16bit(p->dtype, bn, res, splits, m, static_cast<int>(Mrows), p->cout, mt, nkb, g, p->ep, p->workspace,
+                      out, p->ldo, static_cast<cudaStream_t>(stream));
 }
 
-static int conv_check(const mimo_conv3x3_params* p, const char* who) {
+static int conv_check(const mimo_conv3x3_params* p) {
   if (!p || !p->x0 || !p->w || !p->out) return set_error(MIMO_ERR_ARG, "mimo_conv: null pointer");
   if (p->n <= 0 || p->h <= 0 || p->w_ <= 0 || p->cout <= 0 || p->c0 <= 0)
     return set_error(MIMO_ERR_ARG, "mimo_conv: empty problem");
@@ -662,15 +670,12 @@ static int conv_check(const mimo_conv3x3_params* p, const char* who) {
     return set_error(MIMO_ERR_ARG, "mimo_conv: channel counts must be multiples of 8");
   if (p->ep.act == MIMO_ACT_GEGLU) return set_error(MIMO_ERR_ARG, "mimo_conv: GEGLU not supported");
   if (p->ep.residual && (p->ep.ld_res % 8)) return set_error(MIMO_ERR_ARG, "mimo_conv: ld_res % 8 != 0");
-  (void)who;
   return ensure_device();
 }
 
 extern "C" int mimo_conv3x3(const mimo_conv3x3_params* p, void* stream) {
-  if (int rc = conv_check(p, "mimo_conv3x3")) return rc;
-  static const signed char dx[9] = {-1, 0, 1, -1, 0, 1, -1, 0, 1};
-  static const signed char dy[9] = {-1, -1, -1, 0, 0, 0, 1, 1, 1};
-  return conv_launch(p, p->w, 9, dx, dy, p->out, 1, 1, p->w_, p->h, stream);
+  if (int rc = conv_check(p)) return rc;
+  return conv_launch(p, p->w, 9, kTap3x3Dx, kTap3x3Dy, p->out, 1, stream);
 }
 
 // nearest-x2 upsampling followed by a 3x3 / pad 1 convolution, without the upsampled tensor: output pixel (2y+a, 2x+b)
@@ -678,7 +683,7 @@ extern "C" int mimo_conv3x3(const mimo_conv3x3_params* p, void* stream) {
 // 2x2-tap convolution over the SOURCE image whose weights are sums of the 3x3 taps that land on the same source pixel
 // (packed by the host: w = [4 classes][cout, 4 * cin], class = 2a + b, tap = 2 iy + ix). 4/9 of the FLOPs, no 4x buffer.
 extern "C" int mimo_conv_up2x(const mimo_conv3x3_params* p, void* stream) {
-  if (int rc = conv_check(p, "mimo_conv_up2x")) return rc;
+  if (int rc = conv_check(p)) return rc;
   if (p->ep.residual || p->ep.rowvec) return set_error(MIMO_ERR_ARG, "mimo_conv_up2x: bias / activation epilogue only");
   const int ctot = p->c0 + (p->x1 ? p->c1 : 0);
   const size_t esz = 2;
@@ -690,52 +695,9 @@ extern "C" int mimo_conv_up2x(const mimo_conv3x3_params* p, void* stream) {
                                  static_cast<signed char>(a), static_cast<signed char>(a)};
       const char* w = static_cast<const char*>(p->w) + static_cast<size_t>(2 * a + b) * p->cout * 4 * ctot * esz;
       char* out = static_cast<char*>(p->out) + (static_cast<size_t>(a) * 2 * p->w_ + b) * p->ldo * esz;
-      if (int rc = conv_launch(p, w, 4, dx, dy, out, 2, 2, 2 * p->w_, 2 * p->h, stream)) return rc;
+      if (int rc = conv_launch(p, w, 4, dx, dy, out, 2, stream)) return rc;
     }
   return MIMO_OK;
-}
-
-// e4m3 conv tile widths (conv_e4m3_kernel instantiations): 160 divides every ResBlock width (320, 640, 1280), 256 divides
-// 1280. At 1280 BN 256 spills (ptxas report above) and 160 does not; measured on an H100 SXM (700 W) at the 48 images of
-// the 512 x 512 CFG window, 256 was faster where its tiles fit one wave and 160's did not (8 x 8: 66 / 68 / 123 us
-// against 83 / 85 / 152 us), and at 16 x 16 the two were within 8 % either way (scripts/fp8_conv_bench.py). So: 256 when
-// that saves a wave, else the least padded width, 160 on a tie.
-static int pick_bn_conv_e4m3(int N, long long m_tiles) {
-  if (g_force_bn) return g_force_bn;
-  const long long t256 = m_tiles * ((N + 255) / 256), t160 = m_tiles * ((N + 159) / 160);
-  if (N % 256 == 0 && t256 <= num_sms() && t160 > num_sms()) return 256;
-  const int pad256 = (N + 255) / 256 * 256 - N, pad160 = (N + 159) / 160 * 160 - N;
-  return pad256 < pad160 ? 256 : 160;
-}
-
-template <int BN, bool kBf16, bool kRes>
-static int launch_conv_e4m3_cfg(const Maps& m, int M, int N, int mt, int nt, int nkb, const ConvGeom& g,
-                                const EpiArgs& ep, const float* a_scale, const float* w_scale, cudaStream_t st) {
-  constexpr int kSmem = GemmCfg<BN, kRes, true>::kSmemBytes;
-  auto kern = conv_e4m3_kernel<BN, kBf16, kRes>;
-  static bool attr_done = false;  // per instantiation
-  if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
-    if (e != cudaSuccess) return set_cuda_error("cudaFuncSetAttribute(conv_e4m3)", e);
-    attr_done = true;
-  }
-  const int tiles = mt * nt;
-  const int grid = tiles < num_sms() ? tiles : num_sms();
-  cudaError_t e = launch_k(kern, dim3(grid), dim3(kGemmThreads), kSmem, st, m.a0, m.a1, m.b, m.out, m.res, M, N, mt, nt,
-                           nkb, g, ep, a_scale, w_scale);
-  if (e == cudaSuccess) e = cudaGetLastError();
-  if (e != cudaSuccess) return set_cuda_error("conv_e4m3 launch", e);
-  return MIMO_OK;
-}
-
-template <bool kBf16>
-static int launch_conv_e4m3(int bn, bool res, const Maps& m, int M, int N, int mt, int nt, int nkb, const ConvGeom& g,
-                            const EpiArgs& ep, const float* a_scale, const float* w_scale, cudaStream_t st) {
-  if (bn == 160)
-    return res ? launch_conv_e4m3_cfg<160, kBf16, true>(m, M, N, mt, nt, nkb, g, ep, a_scale, w_scale, st)
-               : launch_conv_e4m3_cfg<160, kBf16, false>(m, M, N, mt, nt, nkb, g, ep, a_scale, w_scale, st);
-  return res ? launch_conv_e4m3_cfg<256, kBf16, true>(m, M, N, mt, nt, nkb, g, ep, a_scale, w_scale, st)
-             : launch_conv_e4m3_cfg<256, kBf16, false>(m, M, N, mt, nt, nkb, g, ep, a_scale, w_scale, st);
 }
 
 extern "C" int mimo_conv3x3_e4m3(const mimo_conv3x3_e4m3_params* p, void* stream) {
@@ -753,64 +715,29 @@ extern "C" int mimo_conv3x3_e4m3(const mimo_conv3x3_e4m3_params* p, void* stream
   if (p->workspace || p->workspace_bytes) return set_error(MIMO_ERR_ARG, "mimo_conv3x3_e4m3: split-K is not supported");
   const long long Mrows = static_cast<long long>(p->n) * p->h * p->w_;
   if (Mrows > 0x7fffffffLL) return set_error(MIMO_ERR_ARG, "mimo_conv3x3_e4m3: too many pixels");
-  if (g_force_bn && g_force_bn != 160 && g_force_bn != 256)
+  if (g_force_bn && !WidthsConvE4m3::has(g_force_bn))
     return set_error(MIMO_ERR_ARG, "mimo_conv3x3_e4m3: unsupported BN (160 or 256)");
   if (int rc = ensure_device()) return rc;
 
-  ConvGeom g = {};
-  const int tiles_n = conv_tiles(g, p->n, p->h, p->w_);
-  const int bn = pick_bn_conv_e4m3(p->cout, static_cast<long long>(g.tiles_w) * g.tiles_h * tiles_n);
-  g.ctot = g.c0 = p->c_in;
-  g.kb0 = (p->c_in + 2 * BK - 1) / (2 * BK);  // 128-channel blocks per tap
-  g.a_bytes = g.TW * g.TH * g.TN * 2 * BK;
-  g.chunk_bytes = g.TW * g.TH * g.TN * 64;
-  g.ntaps = 9;
-  for (int t = 0; t < 9; ++t) {
-    g.tdx[t] = static_cast<signed char>(t % 3 - 1);
-    g.tdy[t] = static_cast<signed char>(t / 3 - 1);
-  }
-  const int mt = g.tiles_w * g.tiles_h * tiles_n;
-  const int nkb = 9 * g.kb0;
-  g.splits = 1;
-  g.kb_split = nkb;
+  ConvGeom g;
+  const int mt = conv_geom(g, p->n, p->h, p->w_, p->c_in, 0, 2 * BK, 1, 9, kTap3x3Dx, kTap3x3Dy);
+  const int nkb = g.kb_split;
+  const int bn = pick_bn_conv_e4m3(p->cout, mt);
   const int nt = (p->cout + bn - 1) / bn;
   const bool res = p->ep.residual != nullptr;
 
   Maps m;
-  const uint32_t tile[3] = {static_cast<uint32_t>(g.TW), static_cast<uint32_t>(g.TH), static_cast<uint32_t>(g.TN)};
-  {
-    const uint64_t dim[4] = {static_cast<uint64_t>(p->c_in), static_cast<uint64_t>(p->w_), static_cast<uint64_t>(p->h),
-                             static_cast<uint64_t>(p->n)};
-    const uint64_t str[3] = {static_cast<uint64_t>(p->c_in), static_cast<uint64_t>(p->w_) * p->c_in,
-                             static_cast<uint64_t>(p->h) * p->w_ * p->c_in};
-    const uint32_t box[4] = {2 * BK, tile[0], tile[1], tile[2]};
-    if (int rc = encode_tmap(&m.a0, kTmapU8, 4, p->x, dim, str, box)) return rc;
-    m.a1 = m.a0;
-  }
-  {
-    const uint64_t dim[2] = {9ull * p->c_in, static_cast<uint64_t>(p->cout)};
-    const uint64_t str[1] = {9ull * p->c_in};
-    const uint32_t box[2] = {2 * BK, static_cast<uint32_t>(bn)};
-    if (int rc = encode_tmap(&m.b, kTmapU8, 2, p->w, dim, str, box)) return rc;
-  }
-  auto out_map = [&](CUtensorMap* tm, const void* base, long long pitch) {
-    const uint64_t dim[4] = {static_cast<uint64_t>(p->cout), static_cast<uint64_t>(p->w_), static_cast<uint64_t>(p->h),
-                             static_cast<uint64_t>(p->n)};
-    const uint64_t str[3] = {static_cast<uint64_t>(pitch) * 2, static_cast<uint64_t>(p->w_) * pitch * 2,
-                             static_cast<uint64_t>(p->h) * p->w_ * pitch * 2};
-    const uint32_t box[4] = {32, tile[0], tile[1], tile[2]};
-    return encode_tmap(tm, p->dtype, 4, base, dim, str, box, 64);
-  };
-  if (int rc = out_map(&m.out, p->out, p->ldo)) return rc;
-  m.res = m.out;
-  if (res)
-    if (int rc = out_map(&m.res, p->ep.residual, p->ep.ld_res)) return rc;
+  if (int rc = nhwc_map(&m.a0, kTmapU8, p->x, g, p->c_in, p->c_in, 2 * BK, 128)) return rc;
+  m.a1 = m.a0;
+  if (int rc = rows_map(&m.b, kTmapU8, p->w, 9ull * p->c_in, p->cout, 9ull * p->c_in, 2 * BK, bn)) return rc;
+  if (int rc = out_maps_nhwc(m, p->dtype, g, p->out, p->ldo, 1, p->ep.residual, p->ep.ld_res, p->cout)) return rc;
   const EpiArgs ep = make_epi(p->ep, p->cout);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int M = static_cast<int>(Mrows);
-  return p->dtype == MIMO_BF16
-             ? launch_conv_e4m3<true>(bn, res, m, M, p->cout, mt, nt, nkb, g, ep, p->x_scale, p->w_scale, st)
-             : launch_conv_e4m3<false>(bn, res, m, M, p->cout, mt, nt, nkb, g, ep, p->x_scale, p->w_scale, st);
+  return WidthsConvE4m3::dispatch("conv_e4m3", bn, p->dtype, res, [&](auto kBN, auto kBf16, auto kRes) {
+    return launch_gemm_kernel<conv_e4m3_kernel<kBN, kBf16, kRes>, GemmCfg<kBN, kRes, true>::kSmemBytes>(
+        "conv_e4m3", mt * nt, st, m.a0, m.a1, m.b, m.out, m.res, M, p->cout, mt, nt, nkb, g, ep, p->x_scale, p->w_scale);
+  });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -830,100 +757,33 @@ extern "C" int mimo_gemm_e4m3_geglu_e4m3(const mimo_gemm_e4m3_geglu_e4m3_params*
     return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_geglu_e4m3: a, w, out must be 16-byte aligned");
   if (reinterpret_cast<uintptr_t>(p->out_scale) % 16)
     return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_geglu_e4m3: out_scale must be 16-byte aligned");
-  if (pick_bn(p->N, true, 1 << 20) != 256)
+  const int bn = pick_bn(p->N, true, 1 << 20);
+  if (!WidthsGegluE4m3::has(bn))
     return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_geglu_e4m3: needs the 256-wide GEGLU tile");
   if (int rc = ensure_device()) return rc;
-  constexpr int bn = 256;
   const int mt = (p->M + BM - 1) / BM;
   const int nt = p->N / bn;
   const int nkb = (p->K + 2 * BK - 1) / (2 * BK);
 
   Maps m;
-  const uint64_t adim[2] = {static_cast<uint64_t>(p->K), static_cast<uint64_t>(p->M)};
-  const uint64_t astr[1] = {static_cast<uint64_t>(p->lda)};
-  const uint32_t abox[2] = {2 * BK, BM};
-  if (int rc = encode_tmap(&m.a0, kTmapU8, 2, p->a, adim, astr, abox)) return rc;
+  if (int rc = rows_map(&m.a0, kTmapU8, p->a, p->K, p->M, p->lda, 2 * BK, BM)) return rc;
   m.a1 = m.a0;
-  const uint64_t bdim[2] = {static_cast<uint64_t>(p->K), static_cast<uint64_t>(p->N)};
-  const uint64_t bstr[1] = {static_cast<uint64_t>(p->ldw)};
-  const uint32_t bbox[2] = {2 * BK, static_cast<uint32_t>(bn)};
-  if (int rc = encode_tmap(&m.b, kTmapU8, 2, p->w, bdim, bstr, bbox)) return rc;
+  if (int rc = rows_map(&m.b, kTmapU8, p->w, p->K, p->N, p->ldw, 2 * BK, bn)) return rc;
   // output: one-byte elements, 128-row x 128-column boxes (one 128-byte swizzle row per tile row)
-  const uint64_t odim[2] = {static_cast<uint64_t>(p->N / 2), static_cast<uint64_t>(p->M)};
-  const uint64_t ostr[1] = {static_cast<uint64_t>(p->ldo)};
-  const uint32_t obox[2] = {2 * BK, BM};
-  if (int rc = encode_tmap(&m.out, kTmapU8, 2, p->out, odim, ostr, obox)) return rc;
+  if (int rc = rows_map(&m.out, kTmapU8, p->out, p->N / 2, p->M, p->ldo, 2 * BK, BM)) return rc;
   m.res = m.out;
-  ConvGeom g = {};
-  g.kb0 = nkb;
-  g.c0 = p->K;
-  g.chunk_bytes = kChunk;
-  g.splits = 1;
-  g.kb_split = nkb;
+  const ConvGeom g = gemm_rows(p->K, nkb);
   mimo_epilogue e = {};
   e.bias = p->bias;
   e.scale = 1.0f;
   e.act = MIMO_ACT_GEGLU;
   const EpiArgs ep = make_epi(e, p->N);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  auto run = [&](auto kern, bool& done) -> int {
-    constexpr int smem = GemmCfg<256, false, true>::kSmemBytes;
-    if (!done) {
-      cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-      if (err != cudaSuccess) return set_cuda_error("cudaFuncSetAttribute(gemm_e4m3_geglu_e4m3)", err);
-      done = true;
-    }
-    const int tiles = mt * nt;
-    const int grid = tiles < num_sms() ? tiles : num_sms();
-    cudaError_t err = launch_k(kern, dim3(grid), dim3(kGemmThreads), smem, st, m.a0, m.a1, m.b, m.out, m.res, p->M, p->N,
-                               mt, nt, nkb, g, ep, p->a_scale, p->w_scale, p->out_scale,
-                               static_cast<long long>(p->ld_scale));
-    if (err == cudaSuccess) err = cudaGetLastError();
-    if (err != cudaSuccess) return set_cuda_error("gemm_e4m3_geglu_e4m3 launch", err);
-    return MIMO_OK;
-  };
-  static bool done[2] = {};
-  return p->dtype == MIMO_BF16 ? run(gemm_e4m3_geglu_e4m3_kernel<true>, done[1])
-                               : run(gemm_e4m3_geglu_e4m3_kernel<false>, done[0]);
-}
-
-// block-scaled tile widths (gemm_blockscaled_kernel instantiations): the per-block accumulator doubles the accumulator
-// registers, so 64 and 128 (ptxas report above). Measured on an H100 SXM (700 W) at the FF-out shapes of the 512 x 512
-// CFG window (scripts/fp8_ff_bench.py), 128 was faster at every width, even at N = 320 where it pads to 384 columns
-// (290 against 302 us at 64 x 64: 3 column tiles read each A tile 3 times instead of 5): 128, and 64 only for N <= 64.
-static int pick_bn_blockscaled(int N) {
-  if (g_force_bn) return g_force_bn;
-  return N <= 64 ? 64 : 128;
-}
-
-template <int BN, bool kBf16, bool kRes>
-static int launch_blockscaled_cfg(const Maps& m, const CUtensorMap& tas, int M, int N, int mt, int nt, int nkb,
-                                  const ConvGeom& g, const EpiArgs& ep, const float* w_scale, cudaStream_t st) {
-  constexpr int kSmem = GemmCfg<BN, kRes, true, true>::kSmemBytes;
-  auto kern = gemm_blockscaled_kernel<BN, kBf16, kRes>;
-  static bool attr_done = false;  // per instantiation
-  if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
-    if (e != cudaSuccess) return set_cuda_error("cudaFuncSetAttribute(gemm_blockscaled)", e);
-    attr_done = true;
-  }
-  const int tiles = mt * nt;
-  const int grid = tiles < num_sms() ? tiles : num_sms();
-  cudaError_t e = launch_k(kern, dim3(grid), dim3(kGemmThreads), kSmem, st, m.a0, m.a1, m.b, m.out, m.res, tas, M, N, mt,
-                           nt, nkb, g, ep, w_scale);
-  if (e == cudaSuccess) e = cudaGetLastError();
-  if (e != cudaSuccess) return set_cuda_error("gemm_blockscaled launch", e);
-  return MIMO_OK;
-}
-
-template <bool kBf16>
-static int launch_blockscaled(int bn, bool res, const Maps& m, const CUtensorMap& tas, int M, int N, int mt, int nt,
-                              int nkb, const ConvGeom& g, const EpiArgs& ep, const float* w_scale, cudaStream_t st) {
-  if (bn == 64)
-    return res ? launch_blockscaled_cfg<64, kBf16, true>(m, tas, M, N, mt, nt, nkb, g, ep, w_scale, st)
-               : launch_blockscaled_cfg<64, kBf16, false>(m, tas, M, N, mt, nt, nkb, g, ep, w_scale, st);
-  return res ? launch_blockscaled_cfg<128, kBf16, true>(m, tas, M, N, mt, nt, nkb, g, ep, w_scale, st)
-             : launch_blockscaled_cfg<128, kBf16, false>(m, tas, M, N, mt, nt, nkb, g, ep, w_scale, st);
+  return WidthsGegluE4m3::dispatch("gemm_e4m3_geglu_e4m3", bn, p->dtype, false, [&](auto kBN, auto kBf16, auto) {
+    return launch_gemm_kernel<gemm_e4m3_geglu_e4m3_kernel<kBf16>, GemmCfg<kBN, false, true>::kSmemBytes>(
+        "gemm_e4m3_geglu_e4m3", mt * nt, st, m.a0, m.a1, m.b, m.out, m.res, p->M, p->N, mt, nt, nkb, g, ep, p->a_scale,
+        p->w_scale, p->out_scale, static_cast<long long>(p->ld_scale));
+  });
 }
 
 extern "C" int mimo_gemm_e4m3_blockscaled(const mimo_gemm_e4m3_blockscaled_params* p, void* stream) {
@@ -943,7 +803,7 @@ extern "C" int mimo_gemm_e4m3_blockscaled(const mimo_gemm_e4m3_blockscaled_param
   if (p->ep.act == MIMO_ACT_GEGLU) return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_blockscaled: GEGLU not supported");
   if (p->workspace || p->workspace_bytes)
     return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_blockscaled: split-K is not supported");
-  if (g_force_bn && g_force_bn != 64 && g_force_bn != 128)
+  if (g_force_bn && !WidthsBlockScaled::has(g_force_bn))
     return set_error(MIMO_ERR_ARG, "mimo_gemm_e4m3_blockscaled: unsupported BN (64 or 128)");
   if (int rc = ensure_device()) return rc;
   const int bn = pick_bn_blockscaled(p->N);
@@ -953,41 +813,19 @@ extern "C" int mimo_gemm_e4m3_blockscaled(const mimo_gemm_e4m3_blockscaled_param
   const bool res = p->ep.residual != nullptr;
 
   Maps m;
-  const uint64_t adim[2] = {static_cast<uint64_t>(p->K), static_cast<uint64_t>(p->M)};
-  const uint64_t astr[1] = {static_cast<uint64_t>(p->lda)};
-  const uint32_t abox[2] = {2 * BK, BM};
-  if (int rc = encode_tmap(&m.a0, kTmapU8, 2, p->a, adim, astr, abox)) return rc;
+  if (int rc = rows_map(&m.a0, kTmapU8, p->a, p->K, p->M, p->lda, 2 * BK, BM)) return rc;
   m.a1 = m.a0;
-  const uint64_t bdim[2] = {static_cast<uint64_t>(p->K), static_cast<uint64_t>(p->N)};
-  const uint64_t bstr[1] = {static_cast<uint64_t>(p->ldw)};
-  const uint32_t bbox[2] = {2 * BK, static_cast<uint32_t>(bn)};
-  if (int rc = encode_tmap(&m.b, kTmapU8, 2, p->w, bdim, bstr, bbox)) return rc;
-  const uint64_t odim[2] = {static_cast<uint64_t>(p->N), static_cast<uint64_t>(p->M)};
-  const uint64_t ostr[1] = {static_cast<uint64_t>(p->ldo) * 2};
-  const uint32_t obox[2] = {32, BM};
-  if (int rc = encode_tmap(&m.out, p->dtype, 2, p->out, odim, ostr, obox, 64)) return rc;
-  m.res = m.out;
-  if (res) {
-    const uint64_t rstr[1] = {static_cast<uint64_t>(p->ep.ld_res) * 2};
-    if (int rc = encode_tmap(&m.res, p->dtype, 2, p->ep.residual, odim, rstr, obox, 64)) return rc;
-  }
+  if (int rc = rows_map(&m.b, kTmapU8, p->w, p->K, p->N, p->ldw, 2 * BK, bn)) return rc;
+  if (int rc = out_maps_rows(m, p->dtype, p->out, p->ldo, p->ep.residual, p->ep.ld_res, p->N, p->M)) return rc;
   // row scales: fp32 [K / 128][ld_scale] read as 16-bit pairs, one 128-row (512-byte) box per K block; rows past M
   // are zero-filled
   CUtensorMap tas;
-  {
-    const uint64_t dim[2] = {2ull * p->M, static_cast<uint64_t>(nkb)};
-    const uint64_t str[1] = {static_cast<uint64_t>(p->ld_scale) * 4};
-    const uint32_t box[2] = {2 * BM, 1};
-    if (int rc = encode_tmap(&tas, MIMO_F16, 2, p->a_scale, dim, str, box, 0)) return rc;
-  }
-  ConvGeom g = {};
-  g.kb0 = nkb;
-  g.c0 = p->K;
-  g.chunk_bytes = kChunk;
-  g.splits = 1;
-  g.kb_split = nkb;
+  if (int rc = rows_map(&tas, MIMO_F16, p->a_scale, 2ull * p->M, nkb, p->ld_scale * 4, 2 * BM, 1, 0)) return rc;
+  const ConvGeom g = gemm_rows(p->K, nkb);
   const EpiArgs ep = make_epi(p->ep, p->N);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  return p->dtype == MIMO_BF16 ? launch_blockscaled<true>(bn, res, m, tas, p->M, p->N, mt, nt, nkb, g, ep, p->w_scale, st)
-                               : launch_blockscaled<false>(bn, res, m, tas, p->M, p->N, mt, nt, nkb, g, ep, p->w_scale, st);
+  return WidthsBlockScaled::dispatch("gemm_blockscaled", bn, p->dtype, res, [&](auto kBN, auto kBf16, auto kRes) {
+    return launch_gemm_kernel<gemm_blockscaled_kernel<kBN, kBf16, kRes>, GemmCfg<kBN, kRes, true, true>::kSmemBytes>(
+        "gemm_blockscaled", mt * nt, st, m.a0, m.a1, m.b, m.out, m.res, tas, p->M, p->N, mt, nt, nkb, g, ep, p->w_scale);
+  });
 }

@@ -116,7 +116,8 @@ def test_argument_errors_of_every_compute_entry_point():
     refused(gemm(ldo=63), "multiples of 8")
     refused(gemm(residual=PTR, ld_res=7), "ld_res")
     refused(gemm(act=L.ACT_GEGLU, residual=PTR, ld_res=64), "GEGLU")
-    assert gemm(a1=PTR, K1=12, lda1=16) < 0  # checked after the device probe: "K1/lda1" with a GPU, "no device" here
+    refused(gemm(a1=PTR, K1=12, lda1=16), "K1/lda1")
+    refused(gemm(act=L.ACT_GEGLU, N=72), "N % tile")  # GEGLU tile 64 does not divide N = 72
 
     def conv(fn=lib.mimo_conv3x3, **kw):
         p = L.Conv3x3Params()
